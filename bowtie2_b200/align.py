@@ -82,6 +82,49 @@ def interleave_names(n1, n2):
 
 
 ALL_HITS_CAP = 1024            # records per read kept for -a in exact mode (a warning is printed when a read had more)
+ALL_HITS_CAP_PAIRS = 256      # report entries per pair kept for paired -a
+
+
+def k_caps(options, paired):
+    """entries kept per read (unpaired) or pair (paired) for -k N / -a: N, or 2N + 2 entries per pair (the primaries, then up to N - 1
+    further records of each mate beside the other mate's primary, and an unaligned mate's own record); None outside -k / -a"""
+    if not options or (options.get("k") is None and not options.get("all_hits")):
+        return None
+    if options.get("k") is not None:
+        return int(options["k"]) * 2 + 2 if paired else int(options["k"])
+    return ALL_HITS_CAP_PAIRS if paired else ALL_HITS_CAP
+
+
+def gather_reads(batch, idx):
+    """reads `idx` of a batch (repeats allowed), in that order, as a new ReadBatch"""
+    o = batch.off.astype(np.int64)
+    idx = np.asarray(idx, dtype=np.int64)
+    lens = o[idx + 1] - o[idx]
+    off = np.zeros(len(idx) + 1, dtype=np.uint64)
+    np.cumsum(lens, out=off[1:])
+    src = np.repeat(o[idx] - off[:-1].astype(np.int64), lens) + np.arange(int(off[-1]), dtype=np.int64)
+    return ReadBatch(batch.seq[src], off, None if batch.qual is None else batch.qual[src])
+
+
+def expand_entries(batch, names, res_k, ops_k, cnt, pairs_k=None):
+    """-k / -a entry arrays (bt2g_policy_align_k / _pairs_k, bt2g_xengine_align_k) -> one SAM record per row: each read (pair) repeated
+    once per entry it reports, an unaligned read (a pair) once.  -> (ReadBatch, names, results, ops[, pair records]) for bt2g_sam_format;
+    rows of a pair that are mate context only (found bit 9) are skipped by the formatter."""
+    from .lib import NameTable
+    per = np.maximum(np.asarray(cnt, dtype=np.int64), 1)
+    unit = np.repeat(np.arange(len(per)), per)
+    sub = np.arange(len(unit)) - np.repeat(np.cumsum(per) - per, per)
+    ridx = unit if pairs_k is None else np.stack([2 * unit, 2 * unit + 1], axis=1).reshape(-1)
+    if isinstance(names, NameTable):
+        nm = NameTable(names.rows[ridx])
+    else:
+        lst = list(names)
+        nm = [lst[i] for i in ridx]
+    res_f = np.ascontiguousarray(res_k[unit, sub]).reshape(-1)
+    ops_f = np.ascontiguousarray(ops_k[unit, sub]).reshape(len(ridx), -1)
+    if pairs_k is None:
+        return gather_reads(batch, ridx), nm, res_f, ops_f
+    return gather_reads(batch, ridx), nm, res_f, ops_f, np.ascontiguousarray(pairs_k[unit, sub])
 
 
 def _exact_batch(gpu, batch, names, paired, preset, local, seed, threads=1, options=None):
@@ -105,26 +148,15 @@ def _exact_batch(gpu, batch, names, paired, preset, local, seed, threads=1, opti
             # paired -k N / -a (bt2g_policy_align_pairs_k): entries of two rows per pair (the primaries, then the further concordant pairs
             # or the mates' further alignments beside the opposite primary); rows that are mate context only are skipped by the formatter
             from .lib import policy_align_pairs_k
-            cap = int(options["k"]) * 2 + 2 if options.get("k") is not None else 256
+            cap = k_caps(options, True)
             res_k, ops_k, pairs_k, cnt, truncated, stats = policy_align_pairs_k(gpu._lib, be, prm, batch, names, cap)
             if truncated:
                 sys.stderr.write(f"Warning: -a: pairs with more than {cap} report entries were cut to {cap}\n")
-            per = np.maximum(cnt.astype(np.int64), 1)
-            pidx = np.repeat(np.arange(batch.n // 2), per)
-            sub = np.arange(len(pidx)) - np.repeat(np.cumsum(per) - per, per)
-            o = batch.off.astype(np.int64)
-            nm = list(names)
-            seqs, quals, nms = [], [], []
-            for i in pidx:
-                for r in (2 * i, 2 * i + 1):
-                    seqs.append(batch.seq[o[r]:o[r + 1]]); quals.append(batch.qual[o[r]:o[r + 1]]); nms.append(nm[r])
-            res_f = np.ascontiguousarray(res_k[pidx, sub]).reshape(-1)
-            ops_f = np.ascontiguousarray(ops_k[pidx, sub]).reshape(len(pidx) * 2, -1)
-            return ReadBatch.from_list(seqs, quals), nms, res_f, ops_f, np.ascontiguousarray(pairs_k[pidx, sub]), \
-                (np.ascontiguousarray(res_k[:, 0]).reshape(-1), np.ascontiguousarray(pairs_k[:, 0]))
+            batch_k, names_k, res_f, ops_f, pairs_f = expand_entries(batch, names, res_k, ops_k, cnt, pairs_k)
+            return batch_k, names_k, res_f, ops_f, pairs_f, (np.ascontiguousarray(res_k[:, 0]).reshape(-1), np.ascontiguousarray(pairs_k[:, 0]))
         if multi:
             # unpaired -k N / -a (bt2g_policy_align_k): one record per reported alignment, the read repeated; -a is capped per read
-            cap = int(options["k"]) if options.get("k") is not None else ALL_HITS_CAP
+            cap = k_caps(options, False)
             # the multi-hit arrays are dense (n x cap result rows + n x cap op rows): cut the batch so that they stay under ~4 GiB
             row_bytes = 56 + int(batch.lengths().max() if batch.n else 0) + 64
             max_n = max(1, (4 << 30) // (cap * row_bytes))
@@ -143,15 +175,8 @@ def _exact_batch(gpu, batch, names, paired, preset, local, seed, threads=1, opti
             res_k, ops_k, cnt, truncated, stats = policy_align_k(gpu._lib, be, prm, batch, names, cap)
             if truncated:
                 sys.stderr.write(f"Warning: -a: reads with more than {cap} alignments were cut to {cap} records\n")
-            per = np.maximum(cnt.astype(np.int64), 1)           # an unaligned read still prints one record
-            rows = np.repeat(np.arange(batch.n), per)
-            sub = np.arange(len(rows)) - np.repeat(np.cumsum(per) - per, per)
-            o = batch.off.astype(np.int64)
-            seqs = [batch.seq[o[i]:o[i + 1]] for i in rows]
-            quals = [batch.qual[o[i]:o[i + 1]] for i in rows]
-            nm = list(names)
-            return ReadBatch.from_list(seqs, quals), [nm[i] for i in rows], np.ascontiguousarray(res_k[rows, sub]), np.ascontiguousarray(ops_k[rows, sub]), \
-                np.ascontiguousarray(res_k[:, 0])
+            batch_k, names_k, res_f, ops_f = expand_entries(batch, names, res_k, ops_k, cnt)
+            return batch_k, names_k, res_f, ops_f, np.ascontiguousarray(res_k[:, 0])
         res, ops, pairs, stats = policy_align(gpu._lib, be, prm, batch, names)
     finally:
         pass

@@ -61,8 +61,9 @@ struct XDev {                        // everything the step kernel needs (passed
 	bt2g_read_result *res; uint8_t *resOps; bt2g_pair_result *pairs; uint32_t resMaxOps;
 };
 
-template <typename OFF>
+template <typename OFF, bool K>
 struct DevSvc {
+	static constexpr bool kReport = K;                // the -k / -a report runs after the waves (k_xe_report): keep the report order
 	const DevIndex<OFF> &ix; const bt2g_scoring &sc; const XDev &d;
 	__device__ DevSvc(const DevIndex<OFF> &i, const bt2g_scoring &s, const XDev &dd) : ix(i), sc(s), d(dd) {}
 	__device__ const uint8_t *codes(int read) const { return d.seq + d.roff[read]; }
@@ -159,7 +160,9 @@ __device__ __forceinline__ uint32_t agg_inc(uint32_t *ctr) {
 // The wave runs over the ACTIVE list (activeIn, nAct entries; nullptr = every unit, the first wave): units that wait for an
 // answer append themselves to activeOut, so later waves launch as many threads as there are unfinished units -- the long tail
 // of a batch (a few thousand repeat-rich pairs going through dozens of DP rounds) then occupies a few warps, not the GPU.
-template <typename OFF, int MINB>
+// K: an engine of bt2g_xengine_create_k (the entries are written by k_xe_report after the last wave, not here); the -M build (K false)
+// carries none of the -k / -a report code
+template <typename OFF, int MINB, bool K>
 __global__ void __launch_bounds__(128, MINB) k_xe_step(DevIndex<OFF> ix, bt2g_scoring sc, XParams P, XDev d, const uint32_t *activeIn, uint32_t *activeOut,
                                                        uint32_t nAct, int spread) {
 	// spread = s: one unit per 2^s threads (the others idle).  The state machines of a warp's lanes diverge and serialise, so when
@@ -171,7 +174,7 @@ __global__ void __launch_bounds__(128, MINB) k_xe_step(DevIndex<OFF> ix, bt2g_sc
 	int r = XR_DONE;
 	if(valid) {
 		XUnit &u = d.units[i];
-		DevSvc<OFF> svc(ix, sc, d);
+		DevSvc<OFF, K> svc(ix, sc, d);
 		r = x_step(P, u, svc);
 		switch(r) {
 		case XR_DP: case XR_DP_MATE: {
@@ -194,6 +197,7 @@ __global__ void __launch_bounds__(128, MINB) k_xe_step(DevIndex<OFF> ix, bt2g_sc
 		case XR_DONE: {
 			d.status[i] = 1;
 			agg_inc(&d.q->nDone);
+			if(K) break;
 			const uint64_t r0 = u.paired ? 2 * i : i; const int nr = u.paired ? 2 : 1;
 			for(int k = 0; k < nr; k++) x_fill_result(u, k, svc.codes((int)(r0 + k)), d.res[r0 + k], d.resOps + (r0 + k) * (uint64_t)d.resMaxOps, d.resMaxOps);
 			if(u.paired) { bt2g_pair_result pr; pr.pair_type = u.pairType; pr.kind = u.pairKind; pr.source = 0; pr.score_sum = (int32_t)u.scoreSum; pr.fraglen = u.fraglen; d.pairs[i] = pr; }
@@ -216,6 +220,30 @@ __global__ void __launch_bounds__(128, MINB) k_xe_step(DevIndex<OFF> ix, bt2g_sc
 		if(lane == leader) base = atomicAdd(&d.q->nActive, (uint32_t)__popc(m));
 		base = __shfl_sync(0xffffffffu, base, leader);
 		if(cont) activeOut[base + (uint32_t)__popc(m & ((1u << lane) - 1u))] = (uint32_t)i;
+	}
+}
+
+// -k / -a report: the entries of every unit that finished on the device (status 1), one warp per unit and its lanes over the entries
+// (x_report_entry, shared with the host twin in xengine_host.cpp).  The alignments are read from the units' arenas, which stay valid
+// until the next batch's k_xe_reset.  res: maxPer rows per unit (2 x maxPer paired), ops rows of maxOps bytes, pairs: maxPer per pair.
+__global__ void __launch_bounds__(128) k_xe_report(XParams P, const XUnit *units, const uint8_t *status, uint64_t nUnits, const uint8_t *seq,
+                                                   const uint64_t *roff, uint32_t maxPer, bt2g_read_result *res, uint8_t *ops, uint32_t maxOps,
+                                                   bt2g_pair_result *pairs, uint32_t *nEntries, uint32_t *truncated) {
+	const uint64_t w = (blockIdx.x * (uint64_t)blockDim.x + threadIdx.x) >> 5;
+	const int lane = threadIdx.x & 31;
+	if(w >= nUnits || status[w] != 1) return;
+	const XUnit &u = units[w];
+	const int n = x_report_count(u, P), nw = n < (int)maxPer ? n : (int)maxPer;
+	if(lane == 0) {
+		nEntries[w] = (uint32_t)nw;
+		if(n > (int)maxPer && maxPer > 1) atomicOr(truncated, 1u);
+	}
+	const int per = u.paired ? 2 : 1;
+	const uint64_t r0 = w * (uint64_t)per;
+	const uint8_t *c0 = seq + roff[r0], *c1 = u.paired ? seq + roff[r0 + 1] : nullptr;
+	for(int e = lane; e < (nw > 1 ? nw : 1); e += 32) {
+		const uint64_t ent = w * (uint64_t)maxPer + (uint64_t)e;
+		x_report_entry(u, P, e, c0, c1, res + ent * per, ops + ent * per * (uint64_t)maxOps, maxOps, u.paired ? pairs + ent : nullptr);
 	}
 }
 
@@ -256,6 +284,9 @@ struct bt2g_xengine {
 	cudaEvent_t tev[2][XE_TEV]; int tevN[2] = {0, 0};
 	cudaEvent_t evJoin = nullptr; int dpSideBySide = 1;   // BT2G_XE_DP_SERIAL=1 turns the side-by-side DP launches of small waves off
 	uint64_t launches = 0;             // kernels of this library launched by the last batch
+	// -k / -a engines (bt2g_xengine_create_k): the dense entry arrays of the last batch (d.res / resOps / pairs stay unallocated)
+	uint32_t maxPer = 0;
+	bt2g_read_result *kRes = nullptr; uint8_t *kOps = nullptr; bt2g_pair_result *kPairs = nullptr; uint32_t *kN = nullptr, *kTrunc = nullptr;
 	cudaEvent_t ev[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
 };
 
@@ -345,9 +376,10 @@ int runBatch(bt2g_xengine *e, uint64_t nReads, const char *dNames, uint32_t name
 			uint32_t *out = e->active[(wave + 1) & 1];
 			const int spread = (uint64_t)nAct * 32 <= (uint64_t)e->sms * 2048 * 4 ? 5 : e->bigSpread;       // few units: one per warp
 			const uint64_t nThr = (uint64_t)nAct << spread;
-			if(e->stepOcc >= 8) k_xe_step<OFF, 8><<<grid(nThr, 128), 128, 0, st>>>(ix, e->sc, e->P, d, in, out, nAct, spread);
-			else if(e->stepOcc >= 6) k_xe_step<OFF, 6><<<grid(nThr, 128), 128, 0, st>>>(ix, e->sc, e->P, d, in, out, nAct, spread);
-			else k_xe_step<OFF, 4><<<grid(nThr, 128), 128, 0, st>>>(ix, e->sc, e->P, d, in, out, nAct, spread);
+			if(e->maxPer) k_xe_step<OFF, 4, true><<<grid(nThr, 128), 128, 0, st>>>(ix, e->sc, e->P, d, in, out, nAct, spread);   // (-k / -a: 128 registers)
+			else if(e->stepOcc >= 8) k_xe_step<OFF, 8, false><<<grid(nThr, 128), 128, 0, st>>>(ix, e->sc, e->P, d, in, out, nAct, spread);
+			else if(e->stepOcc >= 6) k_xe_step<OFF, 6, false><<<grid(nThr, 128), 128, 0, st>>>(ix, e->sc, e->P, d, in, out, nAct, spread);
+			else k_xe_step<OFF, 4, false><<<grid(nThr, 128), 128, 0, st>>>(ix, e->sc, e->P, d, in, out, nAct, spread);
 		}
 		cudaEventRecord(ev[1], st);
 		e->launches++;
@@ -403,16 +435,23 @@ int runBatch(bt2g_xengine *e, uint64_t nReads, const char *dNames, uint32_t name
 
 } // namespace
 
-extern "C" {
-
-int bt2g_xengine_create(bt2g_ctx *ctx, const bt2g_policy_params *pp, uint64_t maxUnits, uint32_t maxLen, bt2g_xengine **out) {
-	if(!ctx || !pp || !out || maxUnits == 0 || maxLen == 0) return -1;
-	*out = nullptr;
-	if(!ctx->loaded) { ctx->err = "no index loaded"; return -1; }
-	if(!ctx->info.has_bw || !ctx->info.has_ref) { ctx->err = "xengine: needs the mirror index and the packed reference"; return -1; }
-	if(maxLen > XE_MAX_LEN) { ctx->err = "xengine: reads longer than 512 are not supported"; return -1; }
-	if(pp->all_hits || pp->khits > 1) { ctx->err = "xengine: -k / -a are served by bt2g_policy_align_k"; return -1; }
+// maxPer = 0: one result row per read (bt2g_xengine_create); >= 1: the -k / -a entry arrays (bt2g_xengine_create_k)
+static int createEngine(bt2g_ctx *ctx, const bt2g_policy_params *pp, uint64_t maxUnits, uint32_t maxLen, uint32_t maxPer, bt2g_xengine **out) {
 	BT2G_CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+	if(maxPer) {
+		// the dense arrays: rows of a result and an op string, pair records, entry counts
+		const uint64_t per = pp->paired ? 2 : 1, ents = maxUnits * (uint64_t)maxPer;
+		const uint64_t need = ents * per * (sizeof(bt2g_read_result) + maxLen + 80) + (pp->paired ? ents * sizeof(bt2g_pair_result) : 0) + maxUnits * 4;
+		size_t freeB = 0, totalB = 0;
+		BT2G_CUDA_TRY(ctx, cudaMemGetInfo(&freeB, &totalB));
+		if(need > freeB) {
+			char msg[200];
+			snprintf(msg, sizeof msg, "xengine: the -k / -a report arrays (%.2f GiB for %llu units x %u entries) do not fit the device's free memory (%.2f GiB)",
+			         need / 1073741824.0, (unsigned long long)maxUnits, maxPer, freeB / 1073741824.0);
+			ctx->err = msg;
+			return -2;
+		}
+	}
 	bt2g_xengine *e = new(std::nothrow) bt2g_xengine();
 	if(!e) return -4;
 	e->ctx = ctx; e->pp = *pp; e->maxLen = (int)maxLen; e->maxUnits = maxUnits;
@@ -453,7 +492,15 @@ int bt2g_xengine_create(bt2g_ctx *ctx, const bt2g_policy_params *pp, uint64_t ma
 	rc |= xalloc(e, e->packed, (e->maxBases >> 5) + nR + 2); rc |= xalloc(e, e->nmask, (e->maxBases >> 5) + nR + 2); rc |= xalloc(e, e->nextTask, 1);
 	rc |= xalloc(e, d.q, 1); rc |= xalloc(e, d.units, nU); rc |= xalloc(e, d.status, nU);
 	rc |= xalloc(e, e->active[0], nU); rc |= xalloc(e, e->active[1], nU);
-	rc |= xalloc(e, d.res, nR); rc |= xalloc(e, d.resOps, nR * (uint64_t)e->maxOps); rc |= xalloc(e, d.pairs, nU);
+	if(maxPer) {
+		const uint64_t ents = nU * (uint64_t)maxPer, rows = ents * (pp->paired ? 2 : 1);
+		e->maxPer = maxPer;
+		rc |= xalloc(e, e->kRes, rows); rc |= xalloc(e, e->kOps, rows * (uint64_t)e->maxOps); rc |= xalloc(e, e->kN, nU); rc |= xalloc(e, e->kTrunc, 1);
+		if(pp->paired) rc |= xalloc(e, e->kPairs, ents);
+		d.res = nullptr; d.resOps = nullptr; d.pairs = nullptr;
+	} else {
+		rc |= xalloc(e, d.res, nR); rc |= xalloc(e, d.resOps, nR * (uint64_t)e->maxOps); rc |= xalloc(e, d.pairs, nU);
+	}
 	d.resMaxOps = e->maxOps;
 	if(!rc) {
 		// anchor rectangles: rdlen + 4 * min(maxgap, 15) columns; mate rectangles: the fragment window plus the mate and its gaps
@@ -494,6 +541,29 @@ int bt2g_xengine_create(bt2g_ctx *ctx, const bt2g_policy_params *pp, uint64_t ma
 	return 0;
 }
 
+static int checkCreate(bt2g_ctx *ctx, const bt2g_policy_params *pp, uint64_t maxUnits, uint32_t maxLen, bt2g_xengine **out) {
+	if(!ctx || !pp || !out || maxUnits == 0 || maxLen == 0) return -1;
+	*out = nullptr;
+	if(!ctx->loaded) { ctx->err = "no index loaded"; return -1; }
+	if(!ctx->info.has_bw || !ctx->info.has_ref) { ctx->err = "xengine: needs the mirror index and the packed reference"; return -1; }
+	if(maxLen > XE_MAX_LEN) { ctx->err = "xengine: reads longer than 512 are not supported"; return -1; }
+	return 0;
+}
+
+extern "C" {
+
+int bt2g_xengine_create(bt2g_ctx *ctx, const bt2g_policy_params *pp, uint64_t maxUnits, uint32_t maxLen, bt2g_xengine **out) {
+	if(const int rc = checkCreate(ctx, pp, maxUnits, maxLen, out)) return rc;
+	if(pp->all_hits || pp->khits > 1) { ctx->err = "xengine: -k / -a are served by bt2g_policy_align_k"; return -1; }
+	return createEngine(ctx, pp, maxUnits, maxLen, 0, out);
+}
+
+int bt2g_xengine_create_k(bt2g_ctx *ctx, const bt2g_policy_params *pp, uint64_t maxUnits, uint32_t maxLen, uint32_t maxPerUnit, bt2g_xengine **out) {
+	if(const int rc = checkCreate(ctx, pp, maxUnits, maxLen, out)) return rc;
+	if(maxPerUnit == 0) { ctx->err = "xengine: max_per_unit must be at least 1"; return -1; }
+	return createEngine(ctx, pp, maxUnits, maxLen, maxPerUnit, out);
+}
+
 void bt2g_xengine_destroy(bt2g_xengine *e) {
 	if(!e) return;
 	cudaSetDevice(e->ctx->device);
@@ -508,7 +578,20 @@ void bt2g_xengine_destroy(bt2g_xengine *e) {
 	delete e;
 }
 
-// reads already in device memory; results stay on the device (bt2g_xengine_results_dev).  Units that fall back are re-run
+} // extern "C"
+
+// -k / -a: 1 when the report kernel or the fallback cut a unit's entries (max_per_unit > 1), else 0
+static int finishK(bt2g_xengine *e, cudaStream_t st, bool truncated) {
+	bt2g_ctx *ctx = e->ctx;
+	uint32_t t = 0;
+	BT2G_CUDA_TRY(ctx, cudaMemcpyAsync(&t, e->kTrunc, 4, cudaMemcpyDeviceToHost, st));
+	BT2G_CUDA_TRY(ctx, cudaStreamSynchronize(st));
+	return truncated || t ? 1 : 0;
+}
+
+extern "C" {
+
+// reads already in device memory; results stay on the device (bt2g_xengine_results_dev / _results_k_dev).  Units that fall back are re-run
 // by the coroutine engine over this library's entry points and patched into the device result arrays.
 int bt2g_xengine_run_dev(bt2g_xengine *e, const uint8_t *dSeq, const uint8_t *dQual, const uint64_t *dOff, uint64_t nReads,
                          const char *dNames, uint32_t nameStride, void *stream, uint64_t *stats) {
@@ -523,6 +606,15 @@ int bt2g_xengine_run_dev(bt2g_xengine *e, const uint8_t *dSeq, const uint8_t *dQ
 	e->d.seq = dSeq; e->d.qual = dQual; e->d.roff = dOff;
 	const int rc = ctx->info.off_size == 4 ? runBatch<uint32_t>(e, nReads, dNames, nameStride, st) : runBatch<uint64_t>(e, nReads, dNames, nameStride, st);
 	if(rc) return rc;
+	bool truncated = false;
+	if(e->maxPer) {                                       // -k / -a: the entries of the units that finished on the device
+		const uint64_t nUnits = e->P.paired ? nReads / 2 : nReads;
+		BT2G_CUDA_TRY(ctx, cudaMemsetAsync(e->kTrunc, 0, 4, st));
+		k_xe_report<<<(unsigned)((nUnits * 32 + 127) / 128), 128, 0, st>>>(e->P, e->d.units, e->d.status, nUnits, dSeq, dOff, e->maxPer, e->kRes, e->kOps, e->maxOps,
+		                                                                   e->kPairs, e->kN, e->kTrunc);
+		BT2G_CUDA_TRY(ctx, cudaGetLastError());
+		e->launches++;
+	}
 	if(e->stats[1]) {
 		// fallback units: their reads come back to the host, the coroutine engine answers them through the C ABI
 		// (the coroutine engine drives the context's own entry points and scratch buffers: one fallback at a time per process)
@@ -562,6 +654,28 @@ int bt2g_xengine_run_dev(bt2g_xengine *e, const uint8_t *dSeq, const uint8_t *dQ
 		}
 		for(size_t j = 0; j < ids.size() * per; j++) nptr.push_back(names.data() + j * ns);
 		bt2g_reads sub; sub.n_reads = ids.size() * per; sub.seq = seq.data(); sub.qual = qual.data(); sub.off = soff.data();
+		if(e->maxPer) {
+			// the coroutine engine's entry arrays of the fallback units, spliced into the device arrays unit by unit
+			const uint64_t mp = e->maxPer, rowsU = mp * per;
+			std::vector<bt2g_read_result> res(ids.size() * rowsU); std::vector<uint8_t> ops(res.size() * (size_t)e->maxOps);
+			std::vector<bt2g_pair_result> prs(paired ? ids.size() * mp : 0); std::vector<uint32_t> cnt(ids.size());
+			bt2g_policy_backend be; bt2g_policy_backend_gpu(ctx, &be);
+			bt2g_policy_params pp = e->pp; pp.host_threads = 8;
+			const int rc2 = paired ? bt2g_policy_align_pairs_k(&be, &pp, &sub, nptr.data(), e->maxPer, res.data(), ops.data(), e->maxOps, prs.data(), cnt.data(), nullptr)
+			                       : bt2g_policy_align_k(&be, &pp, &sub, nptr.data(), e->maxPer, res.data(), ops.data(), e->maxOps, cnt.data(), nullptr);
+			if(rc2 < 0) { ctx->err = "xengine: fallback engine failed"; return rc2; }
+			truncated = truncated || rc2 == 1;
+			for(size_t j = 0; j < ids.size(); j++) {
+				const uint64_t r0 = ids[j] * rowsU;
+				BT2G_CUDA_TRY(ctx, cudaMemcpy(e->kRes + r0, res.data() + j * rowsU, rowsU * sizeof(bt2g_read_result), cudaMemcpyHostToDevice));
+				BT2G_CUDA_TRY(ctx, cudaMemcpy(e->kOps + r0 * (uint64_t)e->maxOps, ops.data() + j * rowsU * (size_t)e->maxOps, rowsU * (size_t)e->maxOps, cudaMemcpyHostToDevice));
+				if(paired) BT2G_CUDA_TRY(ctx, cudaMemcpy(e->kPairs + ids[j] * mp, prs.data() + j * mp, mp * sizeof(bt2g_pair_result), cudaMemcpyHostToDevice));
+				BT2G_CUDA_TRY(ctx, cudaMemcpy(e->kN + ids[j], cnt.data() + j, 4, cudaMemcpyHostToDevice));
+			}
+			e->stageMs[6] = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - tFb).count();
+			if(stats) for(int k = 0; k < 8; k++) stats[k] = e->stats[k];
+			return finishK(e, st, truncated);
+		}
 		std::vector<bt2g_read_result> res(sub.n_reads); std::vector<uint8_t> ops(sub.n_reads * (size_t)e->maxOps); std::vector<bt2g_pair_result> prs(ids.size());
 		bt2g_policy_backend be; bt2g_policy_backend_gpu(ctx, &be);
 		bt2g_policy_params pp = e->pp; pp.host_threads = 8;
@@ -576,7 +690,7 @@ int bt2g_xengine_run_dev(bt2g_xengine *e, const uint8_t *dSeq, const uint8_t *dQ
 		e->stageMs[6] = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - tFb).count();
 	}
 	if(stats) for(int k = 0; k < 8; k++) stats[k] = e->stats[k];
-	return 0;
+	return e->maxPer ? finishK(e, st, truncated) : 0;
 }
 
 int bt2g_xengine_streams(bt2g_xengine *e, void **stream, void **stream_hi) {
@@ -602,16 +716,14 @@ int bt2g_xengine_results_dev(bt2g_xengine *e, bt2g_read_result **res, uint8_t **
 	return 0;
 }
 
-// host buffers in, host results out: res[n_reads], ops[n_reads * max_ops] (max_ops >= the engine's own stride is not required:
-// rows are copied with the smaller of the two strides), pairs[n_reads / 2] when paired
-int bt2g_xengine_align(bt2g_xengine *e, const bt2g_reads *reads, const char *names, uint32_t nameStride, bt2g_read_result *res, uint8_t *ops,
-                       uint32_t maxOps, bt2g_pair_result *pairs, uint64_t *stats) {
-	if(!e || !reads || !reads->qual || !res || !ops) return -1;
+} // extern "C"
+
+// bt2g_xengine_align / _align_k: the batch to the device and through its waves; returns bt2g_xengine_run_dev's code, or 2 for an empty batch
+static int runHost(bt2g_xengine *e, const bt2g_reads *reads, const char *names, uint32_t nameStride, uint64_t *stats) {
 	bt2g_ctx *ctx = e->ctx;
 	const uint64_t n = reads->n_reads;
 	if(n > e->maxReads || reads->off[n] > e->maxBases) { ctx->err = "xengine: batch larger than the engine was created for"; return -1; }
-	if(e->P.paired && !pairs) return -1;
-	if(n == 0) return 0;
+	if(n == 0) return 2;
 	for(uint64_t i = 0; i < n; i++)
 		if(reads->off[i + 1] - reads->off[i] > (uint64_t)e->maxLen) { ctx->err = "xengine: a read is longer than the max_len the engine was created for"; return -1; }
 	BT2G_CUDA_TRY(ctx, cudaSetDevice(ctx->device));
@@ -629,13 +741,61 @@ int bt2g_xengine_align(bt2g_xengine *e, const bt2g_reads *reads, const char *nam
 		BT2G_CUDA_TRY(ctx, cudaMemcpyAsync(e->dNames, names, (uint64_t)nameStride * n, cudaMemcpyHostToDevice, st));
 		dn = e->dNames;
 	}
-	const int rc = bt2g_xengine_run_dev(e, e->dSeq, e->dQual, e->dOff, n, dn, nameStride, st, stats);
-	if(rc) return rc;
+	return bt2g_xengine_run_dev(e, e->dSeq, e->dQual, e->dOff, n, dn, nameStride, st, stats);
+}
+
+extern "C" {
+
+// host buffers in, host results out: res[n_reads], ops[n_reads * max_ops] (max_ops >= the engine's own stride is not required:
+// rows are copied with the smaller of the two strides), pairs[n_reads / 2] when paired
+int bt2g_xengine_align(bt2g_xengine *e, const bt2g_reads *reads, const char *names, uint32_t nameStride, bt2g_read_result *res, uint8_t *ops,
+                       uint32_t maxOps, bt2g_pair_result *pairs, uint64_t *stats) {
+	if(!e || !reads || !reads->qual || !res || !ops) return -1;
+	bt2g_ctx *ctx = e->ctx;
+	if(e->P.paired && !pairs) return -1;
+	if(e->maxPer) { ctx->err = "xengine: an engine of bt2g_xengine_create_k reports through bt2g_xengine_align_k"; return -1; }
+	const uint64_t n = reads->n_reads;
+	const int rc = runHost(e, reads, names, nameStride, stats);
+	if(rc) return rc == 2 ? 0 : rc;
+	cudaStream_t st = e->stream;
 	BT2G_CUDA_TRY(ctx, cudaMemcpyAsync(res, e->d.res, n * sizeof(bt2g_read_result), cudaMemcpyDeviceToHost, st));
 	if(maxOps == e->maxOps) BT2G_CUDA_TRY(ctx, cudaMemcpyAsync(ops, e->d.resOps, n * (uint64_t)maxOps, cudaMemcpyDeviceToHost, st));
 	else BT2G_CUDA_TRY(ctx, cudaMemcpy2DAsync(ops, maxOps, e->d.resOps, e->maxOps, maxOps < e->maxOps ? maxOps : e->maxOps, n, cudaMemcpyDeviceToHost, st));
 	if(pairs && e->P.paired) BT2G_CUDA_TRY(ctx, cudaMemcpyAsync(pairs, e->d.pairs, (n / 2) * sizeof(bt2g_pair_result), cudaMemcpyDeviceToHost, st));
 	BT2G_CUDA_TRY(ctx, cudaStreamSynchronize(st));
+	return 0;
+}
+
+// -k / -a: host buffers in, the dense entry arrays out (include/bt2g.h)
+int bt2g_xengine_align_k(bt2g_xengine *e, const bt2g_reads *reads, const char *names, uint32_t nameStride, bt2g_read_result *res, uint8_t *ops,
+                         uint32_t maxOps, bt2g_pair_result *pairs, uint32_t *nEntries, uint64_t *stats) {
+	if(!e || !reads || !reads->qual || !res || !ops || !nEntries) return -1;
+	bt2g_ctx *ctx = e->ctx;
+	if(e->P.paired && !pairs) return -1;
+	if(!e->maxPer) { ctx->err = "xengine: bt2g_xengine_align_k needs an engine of bt2g_xengine_create_k"; return -1; }
+	const uint64_t n = reads->n_reads, nUnits = e->P.paired ? n / 2 : n, ents = nUnits * (uint64_t)e->maxPer, rows = ents * (e->P.paired ? 2 : 1);
+	const int rc = runHost(e, reads, names, nameStride, stats);
+	if(rc < 0) return rc;
+	if(rc == 2) return 0;
+	cudaStream_t st = e->stream;
+	BT2G_CUDA_TRY(ctx, cudaMemcpyAsync(res, e->kRes, rows * sizeof(bt2g_read_result), cudaMemcpyDeviceToHost, st));
+	if(maxOps == e->maxOps) BT2G_CUDA_TRY(ctx, cudaMemcpyAsync(ops, e->kOps, rows * (uint64_t)maxOps, cudaMemcpyDeviceToHost, st));
+	else BT2G_CUDA_TRY(ctx, cudaMemcpy2DAsync(ops, maxOps, e->kOps, e->maxOps, maxOps < e->maxOps ? maxOps : e->maxOps, rows, cudaMemcpyDeviceToHost, st));
+	if(e->P.paired) BT2G_CUDA_TRY(ctx, cudaMemcpyAsync(pairs, e->kPairs, ents * sizeof(bt2g_pair_result), cudaMemcpyDeviceToHost, st));
+	BT2G_CUDA_TRY(ctx, cudaMemcpyAsync(nEntries, e->kN, nUnits * 4, cudaMemcpyDeviceToHost, st));
+	BT2G_CUDA_TRY(ctx, cudaStreamSynchronize(st));
+	return rc;
+}
+
+int bt2g_xengine_results_k_dev(bt2g_xengine *e, bt2g_read_result **res, uint8_t **ops, uint32_t *maxOps, bt2g_pair_result **pairs, uint32_t **nEntries,
+                               uint32_t *maxPerUnit) {
+	if(!e || !e->maxPer) return -1;
+	if(res) *res = e->kRes;
+	if(ops) *ops = e->kOps;
+	if(maxOps) *maxOps = e->maxOps;
+	if(pairs) *pairs = e->kPairs;
+	if(nEntries) *nEntries = e->kN;
+	if(maxPerUnit) *maxPerUnit = e->maxPer;
 	return 0;
 }
 

@@ -511,6 +511,8 @@ XE_HD inline int64_t x_tightened(const XUnit &u, int64_t bestPairScore) {
 //   void extend(int read, bool fw, int rdoff, int seedlen, const uint64_t rng[4], int &nlex, int &nrex)
 //   int ungapped(int read, bool fw, int64_t tidx, int64_t refoff, int64_t tlen, int64_t minsc, bt2g_ungapped_result &r)
 //   int refChar(int64_t tidx, int64_t off)
+//   static constexpr bool kReport: finishRead / finishPair leave the sink lists in report order for x_report_entry (-k / -a);
+//   false compiles the -M-only state machine
 template <typename Svc>
 struct XEngine {
 	const XParams &P; XUnit &u; Svc &svc;
@@ -1318,6 +1320,12 @@ XE_HD inline void x_select(XSel *buf, int n, XRng &rnd) {
 	}
 	if(streak > 1) x_shuffle_portion(buf, n - streak, streak, rnd);
 }
+// -k / -a (Svc::kReport): the sink list(s) rearranged into the selected order (the report order of the secondaries), in place: buf[i].score is
+// free once the caller has read the scores it needs; list b (a concordant pair's mate-2 list) is moved along with list a
+XE_HD inline void x_permute_selected(XSel *buf, int n, uint16_t *a, uint16_t *b) {
+	for(int i = 0; i < n; i++) buf[i].score = (int64_t)a[buf[i].idx] | (b ? (int64_t)b[buf[i].idx] << 16 : 0);
+	for(int i = 0; i < n; i++) { a[i] = (uint16_t)buf[i].score; if(b) b[i] = (uint16_t)(buf[i].score >> 16); }
+}
 
 template <typename Svc>
 XE_HD void XEngine<Svc>::finishPair() {
@@ -1353,6 +1361,7 @@ XE_HD void XEngine<Svc>::finishPair() {
 			const int64_t s2 = a2->refoff - a2->trimLeft(), e2 = a2->refoff + a2->refExtent() + (a2->rdlen - a2->ext() - a2->trimLeft());
 			u.fraglen = (e1 > e2 ? e1 : e2) - (s1 < s2 ? s1 : s2);
 		}
+		if(Svc::kReport && !P.mmode) x_permute_selected(buf, n, u.rs1, u.rs2);
 		return;
 	}
 	if(!u.doneDiscord && u.nunp[0] == 1 && u.nunp[1] == 1) {
@@ -1371,13 +1380,14 @@ XE_HD void XEngine<Svc>::finishPair() {
 		u.resAligned[k] = 1; u.resAln[k] = rsu[buf[0].idx];
 		u.resHasXs[k] = nu > 1; u.resXs[k] = nu > 1 ? x_aln(u, rsu[buf[1].idx])->score : 0;
 		u.resMapq[k] = (int)mapq(x_aln(u, u.resAln[k])->score, u.resHasXs[k] != 0, u.resXs[k], mn[k], u.m[k].perfect);
+		if(Svc::kReport && !P.mmode) x_permute_selected(buf, nu, k == 0 ? u.rs1u : u.rs2u, nullptr);
 		nal++;
 	}
 	u.pairType = nal == 2 ? 2 : (nal == 1 ? 3 : 0);
 }
 
 // ---------------------------------------------------------------------------------------------- single reads
-// multiseedSearchWorker for an unpaired read, as policy_engine.cpp: Engine::readSteps (primary alignment only)
+// multiseedSearchWorker for an unpaired read, as policy_engine.cpp: Engine::readSteps
 template <typename Svc>
 XE_HD int XEngine<Svc>::stepRead() {
 	XMate &c = u.m[0];
@@ -1480,6 +1490,7 @@ XE_HD void XEngine<Svc>::finishRead() {
 	u.resAligned[0] = 1; u.resAln[0] = u.usAlns[buf[0].idx];
 	u.resHasXs[0] = u.nus > 1; u.resXs[0] = u.nus > 1 ? buf[1].score : 0;
 	u.resMapq[0] = (int)mapq(x_aln(u, u.resAln[0])->score, u.resHasXs[0] != 0, u.resXs[0], P.minScore(u.m[0].rdlen), u.m[0].perfect);
+	if(Svc::kReport && !P.mmode) x_permute_selected(buf, u.nus, u.usAlns, nullptr);
 }
 
 // one step of a unit: runs until the next batched request (returned) or the end (XR_DONE)
@@ -1497,18 +1508,75 @@ XE_HD inline void x_unit_reset(XUnit &u, uint32_t id, bool paired) {
 	for(int k = 0; k < 2; k++) { u.resAligned[k] = 0; u.resHasXs[k] = 0; u.resMapq[k] = 0; u.resXs[k] = 0; u.resAln[k] = 0xffff; }
 }
 
-// result of a finished unit -> the pipeline's result arrays (policy_engine.cpp: fillResult)
-XE_HD inline void x_fill_result(const XUnit &u, int k, const uint8_t *codes, bt2g_read_result &out, uint8_t *ops, uint32_t maxOps) {
+// one alignment (or none: an unaligned row) -> a row of the pipeline's result arrays (policy_engine.cpp: fillResult)
+XE_HD inline void x_fill_row(const XAln *a, bool hasXs, int64_t xs, int mapq, const uint8_t *codes, bt2g_read_result &out, uint8_t *ops, uint32_t maxOps) {
 	out.found = 0; out.score = 0; out.score2 = INT32_MIN; out.fw = 0; out.tidx = 0; out.refoff = 0; out.nops = 0; out.ndp = 0;
 	out.trim_left = out.trim_right = 0; out.mapq = 0; out.pad = 0;
-	if(!u.resAligned[k]) return;
-	const XAln *a = x_aln(u, u.resAln[k]);
+	if(!a) return;
 	const int nops = x_aln_to_ops(a, codes, ops, maxOps);
 	out.found = (a->nedits == 0 && a->ext() == a->rdlen) ? 2 : 1;
-	out.score = a->score; if(u.resHasXs[k]) out.score2 = (int32_t)u.resXs[k];
+	out.score = a->score; if(hasXs) out.score2 = (int32_t)xs;
 	out.fw = a->fw; out.tidx = (uint64_t)a->tidx; out.refoff = a->refoff; out.nops = nops;
 	out.trim_left = a->trimLeft(); out.trim_right = a->rdlen - a->ext() - a->trimLeft();
-	out.mapq = u.resMapq[k]; out.pad = a->refns;
+	out.mapq = mapq; out.pad = a->refns;
+}
+// the primary of read k of a finished unit
+XE_HD inline void x_fill_result(const XUnit &u, int k, const uint8_t *codes, bt2g_read_result &out, uint8_t *ops, uint32_t maxOps) {
+	x_fill_row(u.resAligned[k] ? x_aln(u, u.resAln[k]) : nullptr, u.resHasXs[k] != 0, u.resXs[k], u.resMapq[k], codes, out, ops, maxOps);
+}
+
+// ---------------------------------------------------------------------------------------------- -k / -a report
+// The entries of a finished unit in the layout of bt2g_policy_align_k / _pairs_k (policy_engine.cpp: the `finish` lambda of
+// policyAlign).  With Svc::kReport, finishRead / finishPair leave the sink lists in report order outside -M mode, so secondary j of a list is its
+// element j, and ReportingState::getReport (aln_sink.cpp:300-330) reports min(found, khits) of them, the primary included
+// (after a -k short circuit found >= khits).  Under -M every unit reports its primaries only.
+XE_HD inline int x_report_secondaries(const XUnit &u, const XParams &P, int n) {
+	if(P.mmode || n < 1) return 0;
+	return (int)((int64_t)n < P.khits ? (int64_t)n : P.khits) - 1;
+}
+// entries before any cap: unpaired, the primary and its secondaries (0 when unaligned: the unaligned row is written all the same);
+// paired, see x_report_entry
+XE_HD inline int x_report_count(const XUnit &u, const XParams &P) {
+	if(!u.paired) return u.resAligned[0] ? 1 + x_report_secondaries(u, P, u.nus) : 0;
+	if(u.pairType == 1) return 1 + x_report_secondaries(u, P, u.nrs12);
+	const int s0 = u.resAligned[0] ? x_report_secondaries(u, P, u.nrs1u) : 0, s1 = u.resAligned[1] ? x_report_secondaries(u, P, u.nrs2u) : 0;
+	if(s0 + s1 == 0) return 1;
+	return (u.resAligned[0] ? 1 + s0 : 1) + (u.resAligned[1] ? 1 + s1 : 1);
+}
+// entry e of a finished unit: one row (unpaired) or two rows and a pair record (paired), ops rows of maxOps bytes.
+// Paired entries: entry 0 = the primaries; after a concordant pair, the further concordant pairs (both rows secondary); else, when a
+// mate has secondaries, every record of mate 1 and then of mate 2, each beside the opposite mate's primary, an unaligned mate's row
+// last (AlnSinkWrap::finishRead, aln_sink.cpp:930-1010).  found bit 8: secondary (FLAG 256, MAPQ 255, the primary's XS:i);
+// bit 9: the row is there only as its mate's mate.
+XE_HD inline void x_report_entry(const XUnit &u, const XParams &P, int e, const uint8_t *codes0, const uint8_t *codes1, bt2g_read_result *res,
+                                 uint8_t *ops, uint32_t maxOps, bt2g_pair_result *pr) {
+	if(!u.paired) {
+		if(e == 0) { x_fill_result(u, 0, codes0, res[0], ops, maxOps); return; }
+		x_fill_row(x_aln(u, u.usAlns[e]), u.resHasXs[0] != 0, u.resXs[0], 255, codes0, res[0], ops, maxOps);
+		res[0].found |= 0x100;
+		return;
+	}
+	int which[2] = {0, 0}, mark[2] = {0, 0};              // which: 0 = the mate's primary, j > 0 = element j of its report list
+	const uint16_t *list[2] = {u.rs1, u.rs2};
+	if(u.pairType == 1) {
+		if(e > 0) { which[0] = which[1] = e; mark[0] = mark[1] = 0x100; }
+	} else {
+		list[0] = u.rs1u; list[1] = u.rs2u;
+		const int s0 = u.resAligned[0] ? x_report_secondaries(u, P, u.nrs1u) : 0, s1 = u.resAligned[1] ? x_report_secondaries(u, P, u.nrs2u) : 0;
+		if(s0 + s1 > 0) {
+			const int A = u.resAligned[0] ? 1 + s0 : 0, B = u.resAligned[1] ? 1 + s1 : 0;
+			if(e < A) { mark[1] = 0x200; if(e > 0) { which[0] = e; mark[0] = 0x100; } }
+			else if(e - A < B) { mark[0] = 0x200; if(e - A > 0) { which[1] = e - A; mark[1] = 0x100; } }
+			else mark[u.resAligned[0] ? 0 : 1] = 0x200;      // the unaligned mate's own row, beside the aligned mate's primary
+		}
+	}
+	const uint8_t *codes[2] = {codes0, codes1};
+	for(int k = 0; k < 2; k++) {
+		if(which[k]) x_fill_row(x_aln(u, list[k][which[k]]), u.resHasXs[k] != 0, u.resXs[k], 255, codes[k], res[k], ops + (size_t)k * maxOps, maxOps);
+		else x_fill_result(u, k, codes[k], res[k], ops + (size_t)k * maxOps, maxOps);
+		res[k].found |= mark[k];
+	}
+	pr->pair_type = u.pairType; pr->kind = u.pairKind; pr->source = 0; pr->score_sum = (int32_t)u.scoreSum; pr->fraglen = u.fraglen;
 }
 
 } // namespace xe

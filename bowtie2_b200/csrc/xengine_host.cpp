@@ -76,6 +76,7 @@ uint32_t genRandSeed(const uint8_t *codes, const uint8_t *quals, int len, const 
 
 // ---- the services of xengine.cuh answered through the entry-point table, one item per call
 struct HostSvc {
+	static constexpr bool kReport = true;             // (the -M results do not depend on the order of the sink lists)
 	const bt2g_policy_backend &be; const XParams &P; const bt2g_reads *reads; const char *const *names;
 	int rc = 0; uint64_t nCalls = 0;
 	// answers of the batched requests of the unit in flight
@@ -187,10 +188,13 @@ struct HostSvc {
 extern "C" int bt2g_policy_align(const bt2g_policy_backend *, const bt2g_policy_params *, const bt2g_reads *, const char *const *,
                                  bt2g_read_result *, uint8_t *, uint32_t, bt2g_pair_result *, uint64_t *);
 
-extern "C" int bt2g_xengine_align_host(const bt2g_policy_backend *be, const bt2g_policy_params *pp, const bt2g_reads *reads, const char *const *names,
-                                       bt2g_read_result *res, uint8_t *ops, uint32_t maxOps, bt2g_pair_result *pairs, uint64_t *stats) {
+// maxPer = 0: one row per read (bt2g_xengine_align_host); maxPer >= 1: the entry layout of bt2g_policy_align_k / _pairs_k with
+// nEntries[unit] (bt2g_xengine_align_host_k).  Returns 1 when a unit had more entries than maxPer > 1.
+static int alignHost(const bt2g_policy_backend *be, const bt2g_policy_params *pp, const bt2g_reads *reads, const char *const *names, uint32_t maxPer,
+                     bt2g_read_result *res, uint8_t *ops, uint32_t maxOps, bt2g_pair_result *pairs, uint32_t *nEntries, uint64_t *stats) {
 	using namespace xe;
-	if(!be || !pp || !reads || !res || !ops || (pp->paired && (!pairs || (reads->n_reads & 1)))) return -1;
+	if(!be || !pp || !reads || !res || !ops || (pp->paired && (!pairs || (reads->n_reads & 1))) || (maxPer && !nEntries)) return -1;
+	bool truncated = false;
 	int maxLen = 1;
 	for(uint64_t i = 0; i < reads->n_reads; i++) { const int l = (int)(reads->off[i + 1] - reads->off[i]); if(l > maxLen) maxLen = l; }
 	XParams P; XTables T;
@@ -222,10 +226,29 @@ extern "C" int bt2g_xengine_align_host(const bt2g_policy_backend *be, const bt2g
 			uint64_t off3[3] = {0, reads->off[r0 + 1] - reads->off[r0], nr == 2 ? reads->off[r0 + 2] - reads->off[r0] : 0};
 			sub.off = off3;
 			const char *nm[2] = {names ? names[r0] : nullptr, (names && nr == 2) ? names[r0 + 1] : nullptr};
+			if(maxPer) {
+				const size_t e0 = id * (size_t)maxPer;
+				const int rc2 = P.paired ? bt2g_policy_align_pairs_k(be, pp, &sub, names ? nm : nullptr, maxPer, res + 2 * e0, ops + 2 * e0 * (size_t)maxOps, maxOps, pairs + e0, nEntries + id, nullptr)
+				                         : bt2g_policy_align_k(be, pp, &sub, names ? nm : nullptr, maxPer, res + e0, ops + e0 * (size_t)maxOps, maxOps, nEntries + id, nullptr);
+				if(rc2 < 0) return rc2;
+				truncated = truncated || rc2 == 1;
+				continue;
+			}
 			bt2g_pair_result pr{};
 			const int rc2 = bt2g_policy_align(be, pp, &sub, names ? nm : nullptr, res + r0, ops + r0 * (size_t)maxOps, maxOps, P.paired ? &pr : nullptr, nullptr);
 			if(rc2 < 0) return rc2;
 			if(P.paired) pairs[id] = pr;
+			continue;
+		}
+		if(maxPer) {
+			// the same report function as the device engine's k_xe_report, one entry at a time
+			const int n = x_report_count(u, P), nw = n < (int)maxPer ? n : (int)maxPer;
+			truncated = truncated || (n > (int)maxPer && maxPer > 1);
+			const size_t e0 = id * (size_t)maxPer;
+			const uint8_t *c0 = svc.codes((int)r0), *c1 = P.paired ? svc.codes((int)r0 + 1) : nullptr;
+			for(int e = 0; e < (nw > 1 ? nw : 1); e++)
+				x_report_entry(u, P, e, c0, c1, res + (e0 + e) * nr, ops + (e0 + e) * nr * (size_t)maxOps, maxOps, P.paired ? pairs + e0 + e : nullptr);
+			nEntries[id] = (uint32_t)nw;
 			continue;
 		}
 		for(size_t k = 0; k < nr; k++) x_fill_result(u, (int)k, svc.codes((int)(r0 + k)), res[r0 + k], ops + (r0 + k) * (size_t)maxOps, maxOps);
@@ -235,5 +258,17 @@ extern "C" int bt2g_xengine_align_host(const bt2g_policy_backend *be, const bt2g
 		}
 	}
 	if(stats) { stats[0] = units; stats[1] = nFallback; stats[2] = nReq; }
-	return 0;
+	return truncated ? 1 : 0;
+}
+
+extern "C" int bt2g_xengine_align_host(const bt2g_policy_backend *be, const bt2g_policy_params *pp, const bt2g_reads *reads, const char *const *names,
+                                       bt2g_read_result *res, uint8_t *ops, uint32_t maxOps, bt2g_pair_result *pairs, uint64_t *stats) {
+	return alignHost(be, pp, reads, names, 0, res, ops, maxOps, pairs, nullptr, stats);
+}
+
+extern "C" int bt2g_xengine_align_host_k(const bt2g_policy_backend *be, const bt2g_policy_params *pp, const bt2g_reads *reads, const char *const *names,
+                                         uint32_t maxPerUnit, bt2g_read_result *res, uint8_t *ops, uint32_t maxOps, bt2g_pair_result *pairs,
+                                         uint32_t *nEntries, uint64_t *stats) {
+	if(maxPerUnit == 0 || !nEntries) return -1;
+	return alignHost(be, pp, reads, names, maxPerUnit, res, ops, maxOps, pairs, nEntries, stats);
 }

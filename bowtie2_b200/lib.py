@@ -1033,7 +1033,8 @@ class IndexFile:
 
 
 # ---- the exact search policy in waves (include/bt2g.h: bt2g_policy_align; csrc/policy_engine.cpp) ----------------------
-EXPORTS += ["bt2g_policy_align", "bt2g_policy_align_k", "bt2g_policy_align_pairs_k", "bt2g_policy_backend_gpu", "bt2g_xengine_align_host"]
+EXPORTS += ["bt2g_policy_align", "bt2g_policy_align_k", "bt2g_policy_align_pairs_k", "bt2g_policy_backend_gpu", "bt2g_xengine_align_host",
+            "bt2g_xengine_align_host_k"]
 _CB = C.CFUNCTYPE
 _vp = C.c_void_p
 
@@ -1151,6 +1152,33 @@ def policy_align_pairs_k(lib, backend: "_PolicyBackend", params: "_PolicyParams"
     return res[:npairs], ops[:npairs], pairs[:npairs], cnt[:npairs], rc == 1, tuple(int(x) for x in stats)
 
 
+def xengine_align_host_k(lib, backend: "_PolicyBackend", params: "_PolicyParams", reads: ReadBatch, names, max_per_unit: int):
+    """include/bt2g.h: bt2g_xengine_align_host_k (the device engine's state machine and -k / -a report on the host) -> the outputs of
+    policy_align_k (unpaired) or policy_align_pairs_k (paired), stats = (units, fallbacks to the coroutine engine, requests)"""
+    lib.bt2g_xengine_align_host_k.argtypes = [C.POINTER(_PolicyBackend), C.POINTER(_PolicyParams), C.POINTER(_Reads), _vp, C.c_uint32, _vp, _vp,
+                                              C.c_uint32, _vp, _vp, _vp]
+    paired = bool(params.paired)
+    nu = reads.n // 2 if paired else reads.n
+    per = (2,) if paired else ()
+    max_ops = int(reads.lengths().max()) + 64 if reads.n else 64
+    res = np.zeros((max(nu, 1), max_per_unit) + per, dtype=READ_RESULT)
+    ops = np.zeros((max(nu, 1), max_per_unit) + per + (max_ops,), dtype=np.uint8)
+    pairs = np.zeros((max(nu, 1), max_per_unit), dtype=PAIR_RESULT) if paired else None
+    cnt = np.zeros(max(nu, 1), dtype=np.uint32)
+    stats = np.zeros(3, dtype=np.uint64)
+    keep = names.pointers() if isinstance(names, NameTable) else (C.c_char_p * reads.n)(*[x.encode() for x in names])
+    qn = C.cast(keep.ctypes.data if isinstance(names, NameTable) else keep, _vp)
+    st = reads._struct()
+    rc = lib.bt2g_xengine_align_host_k(C.byref(backend), C.byref(params), C.byref(st), qn, int(max_per_unit), _ptr(res), _ptr(ops), max_ops, _ptr(pairs),
+                                       _ptr(cnt), _ptr(stats))
+    if rc < 0:
+        raise RuntimeError(f"bt2g_xengine_align_host_k failed ({rc})")
+    st3 = tuple(int(x) for x in stats)
+    if paired:
+        return res[:nu], ops[:nu], pairs[:nu], cnt[:nu], rc == 1, st3
+    return res[:nu], ops[:nu], cnt[:nu], rc == 1, st3
+
+
 def policy_align_k(lib, backend: "_PolicyBackend", params: "_PolicyParams", reads: ReadBatch, names, max_per_read: int):
     """include/bt2g.h: bt2g_policy_align_k (unpaired -k / -a) -> (results [n, max_per_read], ops [n, max_per_read, max_ops],
     n_reported [n], truncated, (waves, backend calls, requests))"""
@@ -1185,7 +1213,7 @@ def policy_backend_gpu(gpu: "Bt2Gpu") -> "_PolicyBackend":
 
 # ---- the exact search policy on the device (include/bt2g.h: bt2g_xengine_*; csrc/xengine.cuh, xengine.cu) ---------------
 EXPORTS += ["bt2g_xengine_create", "bt2g_xengine_destroy", "bt2g_xengine_align", "bt2g_xengine_run_dev", "bt2g_xengine_results_dev",
-            "bt2g_xengine_stage_ms", "bt2g_xengine_streams"]
+            "bt2g_xengine_stage_ms", "bt2g_xengine_streams", "bt2g_xengine_create_k", "bt2g_xengine_align_k", "bt2g_xengine_results_k_dev"]
 
 XENGINE_STAGES = ("admission", "state_machine", "one_mm", "seed_search", "seed_dp", "mate_dp", "host_fallback", "total", "dp_fill", "dp_tail")
 XENGINE_STATS = ("waves", "fallback_units", "seed_dps", "mate_dps", "seed_dp_cells", "mate_dp_cells", "one_mm_requests", "seed_requests")
@@ -1205,19 +1233,30 @@ def name_rows(names, stride=None) -> np.ndarray:
 
 class XEngine:
     """bt2g_xengine: the reference's search policy as a device-side state machine in waves (records identical to the reference
-    program's).  params: lib.policy_params(...); max_units: pairs (or reads) per call; max_len: longest read."""
+    program's).  params: lib.policy_params(...); max_units: pairs (or reads) per call; max_len: longest read.
+    max_per_unit: None = one row per read (align: the primaries, -M); N = every reported alignment of -k / -a (or -M) in the dense
+    entry layout of policy_align_k / policy_align_pairs_k, up to N entries per read or pair (align_k)."""
 
-    def __init__(self, gpu: "Bt2Gpu", params: "_PolicyParams", max_units: int, max_len: int):
+    def __init__(self, gpu: "Bt2Gpu", params: "_PolicyParams", max_units: int, max_len: int, max_per_unit: int = None):
         self.gpu, self.params, self.max_units, self.max_len = gpu, params, int(max_units), int(max_len)
+        self.max_per_unit = None if max_per_unit is None else int(max_per_unit)
         lib = gpu._lib
         lib.bt2g_xengine_create.argtypes = [_vp, C.POINTER(_PolicyParams), C.c_uint64, C.c_uint32, C.POINTER(_vp)]
+        lib.bt2g_xengine_create_k.argtypes = [_vp, C.POINTER(_PolicyParams), C.c_uint64, C.c_uint32, C.c_uint32, C.POINTER(_vp)]
+        lib.bt2g_xengine_align_k.argtypes = [_vp, C.POINTER(_Reads), _vp, C.c_uint32, _vp, _vp, C.c_uint32, _vp, _vp, _vp]
+        lib.bt2g_xengine_results_k_dev.argtypes = [_vp, C.POINTER(_vp), C.POINTER(_vp), C.POINTER(C.c_uint32), C.POINTER(_vp), C.POINTER(_vp),
+                                                   C.POINTER(C.c_uint32)]
         lib.bt2g_xengine_destroy.argtypes = [_vp]
         lib.bt2g_xengine_destroy.restype = None
         lib.bt2g_xengine_align.argtypes = [_vp, C.POINTER(_Reads), _vp, C.c_uint32, _vp, _vp, C.c_uint32, _vp, _vp]
         lib.bt2g_xengine_run_dev.argtypes = [_vp, _vp, _vp, _vp, C.c_uint64, _vp, C.c_uint32, _vp, _vp]
         lib.bt2g_xengine_results_dev.argtypes = [_vp, C.POINTER(_vp), C.POINTER(_vp), C.POINTER(C.c_uint32), C.POINTER(_vp)]
         h = _vp()
-        gpu._check(lib.bt2g_xengine_create(gpu._h, C.byref(params), self.max_units, self.max_len, C.byref(h)), "bt2g_xengine_create")
+        if self.max_per_unit is None:
+            gpu._check(lib.bt2g_xengine_create(gpu._h, C.byref(params), self.max_units, self.max_len, C.byref(h)), "bt2g_xengine_create")
+        else:
+            gpu._check(lib.bt2g_xengine_create_k(gpu._h, C.byref(params), self.max_units, self.max_len, self.max_per_unit, C.byref(h)),
+                       "bt2g_xengine_create_k")
         self._h = h
         self.paired = bool(params.paired)
         self.max_ops = self.max_len + 80
@@ -1237,12 +1276,36 @@ class XEngine:
                                                          self.max_ops, _ptr(pairs), _ptr(stats)), "bt2g_xengine_align")
         return res, ops, pairs, dict(zip(XENGINE_STATS, (int(x) for x in stats)))
 
-    def run_dev(self, d_seq: int, d_qual: int, d_off: int, n_reads: int, d_names: int = 0, name_stride: int = 0, stream: int = 0):
-        """device pointers in (ints); results stay on the device (results_dev); returns the stats dict"""
+    def align_k(self, reads: ReadBatch, names=None):
+        """-k / -a (an engine made with max_per_unit): host buffers in -> (results [units, max_per_unit] ([.., 2] paired), ops
+        [units, max_per_unit, (2,) max_ops], pair records [units, max_per_unit] or None, n_entries [units], truncated, stats dict).
+        Entries beyond n_entries are not written (an unaligned read's row 0 is)."""
+        if self.max_per_unit is None:
+            raise ValueError("align_k needs an engine created with max_per_unit")
+        nu = reads.n // 2 if self.paired else reads.n
+        per = (2,) if self.paired else ()
+        res = np.empty((nu, self.max_per_unit) + per, dtype=READ_RESULT)
+        ops = np.empty((max(nu, 1), self.max_per_unit) + per + (self.max_ops,), dtype=np.uint8)
+        pairs = np.empty((nu, self.max_per_unit), dtype=PAIR_RESULT) if self.paired else None
+        cnt = np.zeros(max(nu, 1), dtype=np.uint32)
         stats = np.zeros(8, dtype=np.uint64)
-        self.gpu._check(self.gpu._lib.bt2g_xengine_run_dev(self._h, d_seq, d_qual, d_off, n_reads, d_names or None, name_stride, stream or None,
-                                                           _ptr(stats)), "bt2g_xengine_run_dev")
-        return dict(zip(XENGINE_STATS, (int(x) for x in stats)))
+        rows = None if names is None else name_rows(names)
+        st = reads._struct()
+        rc = self.gpu._lib.bt2g_xengine_align_k(self._h, C.byref(st), _ptr(rows), 0 if rows is None else rows.shape[1], _ptr(res), _ptr(ops),
+                                                self.max_ops, _ptr(pairs), _ptr(cnt), _ptr(stats))
+        self.gpu._check(rc if rc < 0 else 0, "bt2g_xengine_align_k")
+        return res, ops[:nu], pairs, cnt[:nu], rc == 1, dict(zip(XENGINE_STATS, (int(x) for x in stats)))
+
+    def run_dev(self, d_seq: int, d_qual: int, d_off: int, n_reads: int, d_names: int = 0, name_stride: int = 0, stream: int = 0):
+        """device pointers in (ints); results stay on the device (results_dev, or results_k_dev for a -k / -a engine); returns the stats
+        dict, with "truncated" for a -k / -a engine (a unit had more entries than max_per_unit > 1: the extra ones were dropped)"""
+        stats = np.zeros(8, dtype=np.uint64)
+        rc = self.gpu._lib.bt2g_xengine_run_dev(self._h, d_seq, d_qual, d_off, n_reads, d_names or None, name_stride, stream or None, _ptr(stats))
+        self.gpu._check(rc if self.max_per_unit is None or rc < 0 else 0, "bt2g_xengine_run_dev")
+        out = dict(zip(XENGINE_STATS, (int(x) for x in stats)))
+        if self.max_per_unit is not None:
+            out["truncated"] = rc == 1
+        return out
 
     def streams(self):
         """(stream, high-priority stream) of the engine as integers (cudaStream_t)"""
@@ -1263,6 +1326,13 @@ class XEngine:
     def launches(self):
         """kernels launched by the last batch (valid after stage_ms())"""
         return getattr(self, "_launches", 0)
+
+    def results_k_dev(self):
+        """-k / -a engine: device pointers (ints) of the entry arrays of the last batch: (res, ops, max_ops, pairs, n_entries, max_per_unit)"""
+        r, o, p, c, m, k = _vp(), _vp(), _vp(), _vp(), C.c_uint32(), C.c_uint32()
+        self.gpu._check(self.gpu._lib.bt2g_xengine_results_k_dev(self._h, C.byref(r), C.byref(o), C.byref(m), C.byref(p), C.byref(c), C.byref(k)),
+                        "bt2g_xengine_results_k_dev")
+        return r.value, o.value, int(m.value), p.value, c.value, int(k.value)
 
     def results_dev(self):
         r, o, p, m = _vp(), _vp(), _vp(), C.c_uint32()

@@ -9,6 +9,7 @@ input order.  This is the batch loop of multiseedSearchWorker (bt2_search.cpp:32
 alignments."""
 import inspect
 import queue
+import sys
 import threading
 
 import numpy as np
@@ -43,8 +44,11 @@ class TextAligner:
     of a batch is handed to the sink as a memoryview of one reused output buffer: the sink must consume it (write it) before it
     returns.  No per-batch allocation is left on the steady-state path."""
 
-    def __init__(self, engines, ref_names, paired, local=False, parse_threads=4, format_threads=8, name_stride=32, depth=2, no_discordant=False, sc=None, make_solo_engine=None):
-        """make_solo_engine: () -> an UNPAIRED engine (same preset and options), created on first use.  A pair whose mate 2 is empty is an
+    def __init__(self, engines, ref_names, paired, local=False, parse_threads=4, format_threads=8, name_stride=32, depth=2, no_discordant=False, sc=None, make_solo_engine=None,
+                 policy_options=None):
+        """policy_options: the run's options; with {"k": N} or {"all_hits": True} the engines (and the solo engine) are -k / -a engines (XEngine
+        with max_per_unit: align_k) and every reported alignment is written, the read or pair repeated per entry (align.expand_entries).
+        make_solo_engine: () -> an UNPAIRED engine (same preset and options), created on first use.  A pair whose mate 2 is empty is an
         unpaired read for the reference (`paired = !read_b().empty()`, bt2_search.cpp:3326: mate 1 goes through the unpaired policy and
         leaves ONE record, YT:Z:UU, counted with the unpaired reads); with the factory those pairs are aligned and written that way,
         without it they stay pairs (two records, mate 2 unaligned with YF:Z:LN)."""
@@ -52,10 +56,11 @@ class TextAligner:
         self.make_solo_engine, self._solo, self._solo_lock = make_solo_engine, None, threading.Lock()
         self.parse_threads, self.format_threads, self.name_stride, self.depth = parse_threads, format_threads, name_stride, depth
         self.no_discordant, self.sc = no_discordant, sc          # the run's --no-discordant / scoring scheme, for the record formatter
+        self.multi = bool(policy_options and (policy_options.get("k") is not None or policy_options.get("all_hits")))
         self.lib = load_library()
         self._slots = [HostBuffers() for _ in range(depth + len(self.engines) + 1)]
         # (engine stand-ins of the CPU tests may not take reusable result buffers)
-        self._reuse = [("out" in inspect.signature(e.align).parameters) for e in self.engines]
+        self._reuse = [(not self.multi and "out" in inspect.signature(e.align).parameters) for e in self.engines]
         self._out = HostBuffers()
 
     def _parse(self, item, slot):
@@ -98,6 +103,69 @@ class TextAligner:
             ops[at:at + len(r), :op.shape[1]] = op
             at += len(r)
         return idx, sb, sn, np.concatenate([p[0] for p in parts]), ops
+
+    @staticmethod
+    def _warn_truncated(eng, paired):
+        cap = eng.max_per_unit
+        if paired:
+            sys.stderr.write(f"Warning: -a: pairs with more than {cap} report entries were cut to {cap}\n")
+        else:
+            sys.stderr.write(f"Warning: -a: reads with more than {cap} alignments were cut to {cap} records\n")
+
+    def _k_segments(self, eng, batch, names):
+        """-k / -a: the batch through align_k, expanded to one record per row, as the formatter's segments (ReadBatch, names, res, ops,
+        pairs or None, primary results and pair records for the alignment counts: entry 0 of every unit), in input order"""
+        from .align import expand_entries
+        res, ops, pairs, cnt, truncated, _ = eng.align_k(batch, names)
+        if truncated:
+            self._warn_truncated(eng, self.paired)
+        if not self.paired:
+            return [(*expand_entries(batch, names, res, ops, cnt), None, np.ascontiguousarray(res[:, 0]), None)]
+        solo = None
+        if self.make_solo_engine is not None:
+            idx = np.nonzero(batch.lengths()[1::2] == 0)[0]
+            if len(idx):
+                solo = (idx, *self._align_solos_k(batch, names, idx))
+        o = batch.off.astype(np.int64)
+
+        def pairs_run(a, b):                                     # pairs [a, b)
+            sb = ReadBatch(batch.seq[o[2 * a]:o[2 * b]], (batch.off[2 * a:2 * b + 1] - batch.off[2 * a]).astype(np.uint64), batch.qual[o[2 * a]:o[2 * b]])
+            return (*expand_entries(sb, names[2 * a:2 * b], res[a:b], ops[a:b], cnt[a:b], pairs[a:b]),
+                    np.ascontiguousarray(res[a:b, 0]).reshape(-1), np.ascontiguousarray(pairs[a:b, 0]))
+        if solo is None:
+            return [pairs_run(0, batch.n // 2)]
+        idx, sb, sn, sres, sops, scnt = solo
+        so = sb.off.astype(np.int64)
+        segs, prev = [], 0
+        for j, p in enumerate(int(x) for x in idx):
+            if p > prev:
+                segs.append(pairs_run(prev, p))
+            one = ReadBatch(sb.seq[so[j]:so[j + 1]], (sb.off[j:j + 2] - sb.off[j]).astype(np.uint64), sb.qual[so[j]:so[j + 1]])
+            segs.append((*expand_entries(one, sn[j:j + 1], sres[j:j + 1], sops[j:j + 1], scnt[j:j + 1]), None, np.ascontiguousarray(sres[j:j + 1, 0]), None))
+            prev = p + 1
+        if prev < batch.n // 2:
+            segs.append(pairs_run(prev, batch.n // 2))
+        return segs
+
+    def _align_solos_k(self, batch, names, idx):
+        """-k / -a: mate 1 of the pairs `idx` (empty mate 2) through the unpaired solo engine: (ReadBatch, names, res, ops, n_entries)"""
+        o = batch.off.astype(np.int64)
+        sb = ReadBatch.from_list([batch.seq[o[2 * i]:o[2 * i + 1]] for i in idx], [batch.qual[o[2 * i]:o[2 * i + 1]] for i in idx])
+        sn = NameTable(np.ascontiguousarray(names.rows[2 * idx])) if isinstance(names, NameTable) else [names[2 * int(i)] for i in idx]
+        with self._solo_lock:
+            if self._solo is None:
+                self._solo = self.make_solo_engine()
+            cap = int(getattr(self._solo, "max_units", 1 << 30))
+            parts = []
+            for a in range(0, sb.n, cap):
+                b = min(sb.n, a + cap)
+                so = sb.off.astype(np.int64)
+                part = ReadBatch(sb.seq[so[a]:so[b]], (sb.off[a:b + 1] - sb.off[a]).astype(np.uint64), sb.qual[so[a]:so[b]])
+                r, op, _, cnt, truncated, _ = self._solo.align_k(part, sn[a:b])
+                if truncated:
+                    self._warn_truncated(self._solo, False)
+                parts.append((r, op, cnt))
+        return sb, sn, np.concatenate([p[0] for p in parts]), np.concatenate([p[1] for p in parts]), np.concatenate([p[2] for p in parts])
 
     @staticmethod
     def _segments(batch, names, res, ops, pairs, solo):
@@ -162,6 +230,9 @@ class TextAligner:
                     if w is END:
                         break
                     k, slot, batch, names = w
+                    if self.multi:                               # -k / -a: segments of expanded records, ready for the formatter
+                        q_done.put((k, slot, batch, names, None, None, None, self._k_segments(eng, batch, names)))
+                        continue
                     res, ops, pairs, _ = eng.align(batch, names, out=slot) if reuse else eng.align(batch, names)
                     solo = self._align_solos(batch, names) if self.paired and self.make_solo_engine is not None else None
                     q_done.put((k, slot, batch, names, res, ops, pairs, solo))
@@ -181,11 +252,16 @@ class TextAligner:
                     pending[w[0]] = w[1:]
                     while nxt in pending:
                         slot, batch, names, res, ops, pairs, solo = pending.pop(nxt)
-                        for b_, n_, r_, o_, p_ in ([(batch, names, res, ops, pairs)] if solo is None else self._segments(batch, names, res, ops, pairs, solo)):
+                        if res is None:                          # -k / -a: the aligner's segments (counted by their primaries)
+                            segs = solo
+                        else:
+                            segs = [(batch, names, res, ops, pairs)] if solo is None else self._segments(batch, names, res, ops, pairs, solo)
+                            segs = [(*sg, sg[2], sg[4]) for sg in segs]
+                        for b_, n_, r_, o_, p_, cr_, cp_ in segs:
                             txt = sam_format(self.lib, b_, r_, o_, self.ref_names, read_names=n_, pairs=p_, threads=self.format_threads,
                                              local=self.local, as_bytes="view", out=self._out, no_discordant=self.no_discordant, sc=self.sc)
                             if on_batch is not None:
-                                on_batch(r_, p_)
+                                on_batch(cr_, cp_)
                             sink(txt)
                         total[0] += batch.n
                         nxt += 1
@@ -272,17 +348,23 @@ def align_files_stream(index_base, out_path, reads1, reads2=None, preset="sensit
                        gpu=None, make_engine=None):
     """bowtie2 -x index_base (-U reads1 | -1 reads1 -2 reads2) -S out_path through the device engine (bt2g_xengine_*: records identical
     to the reference program's) with the host stages overlapped (TextAligner): file blocks are parsed, aligned by `engines` engines on
-    their own streams and host threads, formatted and written in input order.  The primary alignment per read / pair is reported
-    (-M mode; -k / -a are align.align_files(exact=True)'s).  policy_options: keyword arguments of lib.policy_params (nofw, norc, mixed,
-    discord, pe, sc, mhits, seed_len ...).  name_stride: bytes kept per read name (a longer header line is an error, not a silent cut).
+    their own streams and host threads, formatted and written in input order.  The primary alignment per read / pair is reported (-M
+    mode), or with policy_options {"k": N} / {"all_hits": True} every alignment of -k N / -a: the engines keep up to N entries per read
+    (2N + 2 per pair; -a: align.ALL_HITS_CAP / ALL_HITS_CAP_PAIRS, with batch_units cut so that an engine's dense entry arrays stay under
+    about 4 GiB, and a warning when a read had more).  policy_options: keyword arguments of lib.policy_params (nofw, norc, mixed,
+    discord, pe, sc, mhits, seed_len, k, all_hits ...).  name_stride: bytes kept per read name (a longer header line is an error, not a silent cut).
     Returns the ALIGN_COUNTS record; `summary` (a text stream) receives the alignment summary.
     gpu / make_engine: an open Bt2Gpu with the index loaded / a factory (params, max_units, max_len) -> engine, for callers that keep
-    them (and for the CPU tests' stand-ins)."""
+    them (and for the CPU tests' stand-ins); under -k / -a it is called with max_per_unit=... as well."""
+    from .align import k_caps
     from .lib import ALIGN_COUNTS, Bt2Gpu, IndexFile, XEngine, align_counts_add, align_summary, policy_params, sam_header
     opts = dict(policy_options or {})
-    if opts.get("k") is not None or opts.get("all_hits"):
-        raise ValueError("-k / -a are not in the device engine's reporting mode: use align.align_files(exact=True)")
     paired = reads2 is not None
+    cap, solo_cap = k_caps(opts, paired), k_caps(opts, False)
+    if cap is not None:
+        # the entry arrays are dense (units x cap rows of a result and an op string, x 2 for pairs): at most ~4 GiB per engine
+        row_bytes = 56 + max_read_len + 80 + (12 if paired else 0)
+        batch_units = max(1, min(batch_units, (4 << 30) // (cap * (2 if paired else 1) * row_bytes)))
     own = gpu is None
     image = IndexFile(index_base, offrate)
     ref_names, ref_lens = image.ref_names, image.ref_lens
@@ -296,17 +378,18 @@ def align_files_stream(index_base, out_path, reads1, reads2=None, preset="sensit
     image.close()
     lib = load_library()
     prm = policy_params(preset, local=local, paired=paired, seed=seed, host_threads=threads, **opts)
-    make_engine = make_engine or (lambda p, n, l: XEngine(gpu, p, n, l))
-    engs = [make_engine(prm, batch_units, max_read_len) for _ in range(max(1, engines))]
+    make_engine = make_engine or (lambda p, n, l, **kw: XEngine(gpu, p, n, l, **kw))
+    kcap = (lambda c: {} if c is None else {"max_per_unit": c})
+    engs = [make_engine(prm, batch_units, max_read_len, **kcap(cap)) for _ in range(max(1, engines))]
     no_disc, no_mixed = opts.get("discord") is False, opts.get("mixed") is False
     solo_opts = {k: v for k, v in opts.items() if k not in ("pe", "mixed", "discord")}      # the unpaired policy of the same run
     counts = np.zeros(1, dtype=ALIGN_COUNTS)
     src = FastqFiles(reads1, reads2, units=batch_units)
     pthr = max(1, threads // 4)
     ta = TextAligner(engs, [n.split()[0] if n.split() else n for n in ref_names], paired, local=local, parse_threads=pthr,
-                     format_threads=max(1, threads - pthr), name_stride=name_stride, no_discordant=no_disc, sc=opts.get("sc"),
+                     format_threads=max(1, threads - pthr), name_stride=name_stride, no_discordant=no_disc, sc=opts.get("sc"), policy_options=opts,
                      make_solo_engine=(lambda: make_engine(policy_params(preset, local=local, paired=False, seed=seed, host_threads=threads, **solo_opts),
-                                                           min(batch_units, 4096), max_read_len)) if paired else None)
+                                                           min(batch_units, 4096), max_read_len, **kcap(solo_cap))) if paired else None)
     try:
         with open(out_path, "wb") as out:
             out.write(sam_header(lib, ref_names, ref_lens, pg_cl).encode())

@@ -594,7 +594,8 @@ int bt2g_policy_align_pairs_k(const bt2g_policy_backend *be, const bt2g_policy_p
  * kernel (csrc/xengine.cuh / xengine.cu: one thread per read pair or read, state in HBM) and the batched primitives consume
  * device-side request queues once per wave: no host round trip per request, the host only reads the queue counters of each wave.
  * This is the entry point the restated multiseedSearchWorker loop (bt2_search.cpp:3094-4254) calls per block of reads.
- * Supported: the default reporting mode (-M; no -k / -a), end-to-end and --local, paired and unpaired, reads up to 512 bp.
+ * Supported: the default reporting mode (-M) here, -k N / -a through bt2g_xengine_create_k below, end-to-end and --local, paired and
+ * unpaired, reads up to 512 bp.
  * A unit whose state outgrows its fixed capacity is re-run by bt2g_policy_align over bt2g_policy_backend_gpu (same results).
  * create installs the scoring scheme of `prm` in the context (bt2g_set_scoring). */
 typedef struct bt2g_xengine bt2g_xengine;
@@ -624,6 +625,27 @@ int  bt2g_xengine_stage_ms(bt2g_xengine *e, float *ms, uint64_t *launches);
 int  bt2g_xengine_align_host(const bt2g_policy_backend *be, const bt2g_policy_params *prm, const bt2g_reads *reads, const char *const *names,
                              bt2g_read_result *res, uint8_t *ops, uint32_t max_ops, bt2g_pair_result *pairs, uint64_t *stats);
 
+/* -k N / -a (and -M) on the device engine: every reported alignment, in the entry layout of bt2g_policy_align_k (unpaired: rows
+ * [i * max_per_unit, i * max_per_unit + n_entries[i]), an unaligned read has n_entries 0 and an unaligned row at i * max_per_unit) and
+ * bt2g_policy_align_pairs_k (paired: entry e of pair i = rows 2 * (i * max_per_unit + e) + {0, 1} and pairs[i * max_per_unit + e]).
+ * The arrays are byte-identical to those of the coroutine engine over the same primitives.  A kernel (k_xe_report, one warp per
+ * unit) writes the entries after a batch's last wave; units that fall back are re-run by bt2g_policy_align_k / _pairs_k over
+ * bt2g_policy_backend_gpu and spliced in.  create_k accepts any reporting mode and sizes the dense arrays for max_units units
+ * (-2 with the size in err when they do not fit).  align_k: host buffers as bt2g_xengine_align; res[n_units * max_per_unit * (2 if
+ * paired)], ops[rows * max_ops], pairs[n_units * max_per_unit] (paired), n_entries[n_units]; returns 0, 1 when a unit had more
+ * entries than max_per_unit (> 1; the extra ones are dropped), < 0 on error.  bt2g_xengine_run_dev on such an engine leaves them
+ * on the device (and returns 1 on truncation); results_k_dev: those device arrays of the last batch (rows of *max_ops bytes).  bt2g_xengine_align_host_k: the same state machine and report function on the host over an
+ * entry-point table (the CPU pinning), outputs as bt2g_policy_align_k / _pairs_k. */
+int  bt2g_xengine_create_k(bt2g_ctx *ctx, const bt2g_policy_params *prm, uint64_t max_units, uint32_t max_len, uint32_t max_per_unit,
+                           bt2g_xengine **out);
+int  bt2g_xengine_align_k(bt2g_xengine *e, const bt2g_reads *reads, const char *names, uint32_t name_stride, bt2g_read_result *res,
+                          uint8_t *ops, uint32_t max_ops, bt2g_pair_result *pairs, uint32_t *n_entries, uint64_t *stats);
+int  bt2g_xengine_results_k_dev(bt2g_xengine *e, bt2g_read_result **res, uint8_t **ops, uint32_t *max_ops, bt2g_pair_result **pairs,
+                                uint32_t **n_entries, uint32_t *max_per_unit);
+int  bt2g_xengine_align_host_k(const bt2g_policy_backend *be, const bt2g_policy_params *prm, const bt2g_reads *reads, const char *const *names,
+                               uint32_t max_per_unit, bt2g_read_result *res, uint8_t *ops, uint32_t max_ops, bt2g_pair_result *pairs,
+                               uint32_t *n_entries, uint64_t *stats);
+
 /* bt2g_fastq_parse on `threads` host threads: the text is cut at record boundaries, the pieces parsed concurrently and
  * concatenated in input order; outputs, limits and error codes as bt2g_fastq_parse */
 int bt2g_fastq_parse_mt(const char *text, uint64_t len, uint64_t max_reads, uint64_t max_bases, uint8_t *seq, uint8_t *qual,
@@ -647,7 +669,8 @@ int bt2g_fastq_parse_pairs_mt(const char *text1, uint64_t len1, const char *text
  * the reader thread calls next_block and parses (parse_threads), one thread per engine calls `align`, the writer thread formats
  * (format_threads), adds the block to the alignment counts and calls write -- blocks leave in input order, each block in flight
  * owns one set of reused host buffers (depth + n_engines + 1 sets).
- *   align: bt2g_xengine_align itself (cast; engines[j] = a bt2g_xengine*), or any function of that shape.
+ *   align: bt2g_xengine_align itself (cast; engines[j] = a bt2g_xengine*), or any function of that shape: one result row per read, the
+ *     -M reporting mode only (the -k / -a entry arrays of bt2g_xengine_align_k do not fit this loop; stream.py's TextAligner writes them).
  *   next_block: 1 = a block of WHOLE records (at most max_units reads or pairs; paired: the same number of records in both texts,
  *     *text2 / *len2 ignored otherwise), 0 = end of input, < 0 = error; the texts must stay valid until the next call of next_block.
  *   write: SAM records (no header: bt2g_sam_header), valid until write returns; 0 = ok.  One call per block -- more for a block with solo
