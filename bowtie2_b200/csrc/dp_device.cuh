@@ -34,11 +34,13 @@ static inline int dp_rows_per_lane(int maxLen, int mode) {
 // Mode 3 fills row blocks of 32 lanes x DP_BLOCK_RPL rows (k_dp_fill_h); a block takes at most maxCol + 31 steps.
 #define DP_BLOCK_RPL 2
 // bytes of workspace per problem (per warp slot in modes 0-2): (maxCol + 32) steps x 32 lanes x R rows; in mode 3 R rounds up
-// to whole row blocks, and the 32 R bytes the blocks leave free hold their range table
+// to whole row blocks and a block has room for maxCol + 36 steps: the 5 steps per block the blocks leave free hold their range
+// table and the up to 3 steps past the last block's end that the fill's last group of steps stores
 static inline uint64_t dp_code_stride(int maxCol, int maxLen, int mode) {
 	int R = dp_rows_per_lane(maxLen, mode);
 	if(mode == 3) R = (R + DP_BLOCK_RPL - 1) / DP_BLOCK_RPL * DP_BLOCK_RPL;
-	return (((uint64_t)(maxCol + 32) * 32 * (uint64_t)R) + 255) & ~(uint64_t)255;   // planes of hb_index, 256 B aligned
+	const uint64_t steps = (uint64_t)maxCol + (mode == 3 ? 36 : 32);
+	return ((steps * 32 * (uint64_t)R) + 255) & ~(uint64_t)255;   // planes of hb_index, 256 B aligned
 }
 
 // mode 3 workspace: as many problems per chunk as fit a byte budget (default 6 GiB; BT2G_DP_CHUNK_MB overrides)

@@ -770,11 +770,13 @@ __global__ void __launch_bounds__(128, R == 4 ? 6 : 4) k_dp_e2e_h(DevIndex<OFF> 
 #define DP_BLK_MAX (DP_BLK_HEAD / 4)
 static_assert(16 * 32 <= DP_BLK_MAX * DP_BLK_ROWS, "the range table must cover reads of 32 x 16 rows");
 
-// shared memory per warp of k_dp_fill_h: two reference windows, the query profile of one block and the boundary row
-// (OFFDOM: bytes h_A h_B f_A f_B per column, the stored-domain scores being 0..127; otherwise the H and F pairs)
+// shared memory per warp of k_dp_fill_h: two reference windows (each with DP_FILL_PAD columns of padding on either side), the
+// query profile of one block and the boundary row (OFFDOM: bytes h_A h_B f_A f_B per column, the stored-domain scores being
+// 0..127; otherwise the H and F pairs)
+#define DP_FILL_PAD 64
 __host__ __device__ __forceinline__ size_t dp_fill_smem_per_warp(int maxCol, bool offdom) {
 	const size_t win = ((size_t)maxCol + 15) & ~(size_t)15;
-	return 2 * win + DP_QPROF_BYTES(DP_BLOCK_RPL) + win * (offdom ? 4 : 8);
+	return 2 * (win + 2 * DP_FILL_PAD) + DP_QPROF_BYTES(DP_BLOCK_RPL) + win * (offdom ? 4 : 8);
 }
 
 template <bool B> struct DpBool { static constexpr bool value = B; };
@@ -796,14 +798,17 @@ __global__ void __launch_bounds__(128, 8) k_dp_fill_h(DevIndex<OFF> ix, bt2g_sco
 	// shared-memory loads and one IMAD instead of five ALU-pipe instructions -- the ALU pipe is what bounds this kernel
 	const size_t win = ((size_t)L.maxCol + 15) & ~(size_t)15;
 	uint8_t *sm0 = smem + (size_t)warpInBlock * dp_fill_smem_per_warp(L.maxCol, OFFDOM);
-	uint8_t *refw[2] = {sm0, sm0 + win}; uint8_t *hb[2];
+	// every lane computes at every step (see the sweep), so a lane before its first or past its last column reads the windows
+	// up to 31 + 3 columns outside them: the padding holds valid codes (4), set once here; every column ever written is 0..4
+	uint8_t *refw[2] = {sm0 + DP_FILL_PAD, sm0 + win + 3 * DP_FILL_PAD}; uint8_t *hb[2];
+	for(int k = lane; k < 2 * ((int)win + 2 * DP_FILL_PAD); k += 32) sm0[k] = 4;
 	// one 32-bit word per entry, [refc][row-in-lane][lane]: lane k always hits bank k whatever its reference character, so the
 	// look-ups are conflict-free.  A word holds problem A's score in its low half and problem B's in its high half; the packed
 	// pair of a cell is a bit-select of the words its two reference characters pick
-	uint32_t *qprof = reinterpret_cast<uint32_t *>(sm0 + 2 * win);
+	uint32_t *qprof = reinterpret_cast<uint32_t *>(sm0 + 2 * (win + 2 * DP_FILL_PAD));
 	// the last row of the previous block, overwritten in place by the current one: lane 0 reads column c at step c - lo,
 	// lane 31 stores the block's own last row of column c 31 steps later
-	uint32_t *bnd = reinterpret_cast<uint32_t *>(sm0 + 2 * win + DP_QPROF_BYTES(RPL));
+	uint32_t *bnd = reinterpret_cast<uint32_t *>(sm0 + 2 * (win + 2 * DP_FILL_PAD) + DP_QPROF_BYTES(RPL));
 	const int rdgapo = sc.rdgap_const + sc.rdgap_linear, rdgape = sc.rdgap_linear;
 	const int rfgapo = sc.rfgap_const + sc.rfgap_linear, rfgape = sc.rfgap_linear;
 	const int bonus = sc.match_bonus;
@@ -934,8 +939,14 @@ __global__ void __launch_bounds__(128, 8) k_dp_fill_h(DevIndex<OFF> ix, bt2g_sco
 								}
 								if(lane == 0) { inH = bh; inF = bf; }
 							}
-							if((unsigned)(t - lane) < (unsigned)lim) {
-								const int j = lo + t - lane;
+							// Under OFFDOM every lane computes at every step and only the stores depend on the lane's range, so a step is
+							// straight-line code.  That is exact: a lane before its first column only ever sees the initial zeros of the lanes
+							// above it (also not started), and every increment is <= 0, so it keeps its initial zeros; a lane past its last
+							// column feeds only lanes that are past theirs too.  With a match bonus an early lane would climb above its
+							// initial values, so it keeps out of range.
+							const bool on = (unsigned)(t - lane) < (unsigned)lim;
+							if(OFFDOM || on) {
+								const int j = lo + t - lane;             // -31 .. ncolMax + 33: inside the windows' padding
 								const uint32_t *qa = qprof + (int)refw[0][j] * (RPL * 32) + lane, *qb = qprof + (int)refw[1][j] * (RPL * 32) + lane;
 								// H[i0-1][j-1]: row -1 is the free start row of end-to-end mode (vhilsw, :853,923-927)
 								uint32_t diag = (TOP && lane == 0) ? (OFFDOM ? nfloorP : 0u) : prevInH;
@@ -957,17 +968,22 @@ __global__ void __launch_bounds__(128, 8) k_dp_fill_h(DevIndex<OFF> ix, bt2g_sco
 								}
 								botH = upH; botF = upF;
 								prevInH = inH;
-								// byte 0 of every word is problem A's cell, byte 2 problem B's
-								if(RPL == 2) {
-									const uint32_t w2 = __byte_perm(hs[0], hs[RPL - 1], 0x6240);
-									*reinterpret_cast<uint16_t *>(dA + u * 32 * RPL) = (uint16_t)w2;
-									*reinterpret_cast<uint16_t *>(dB + u * 32 * RPL) = (uint16_t)(w2 >> 16);
-								} else {
-									dA[u * 32 * RPL] = (uint8_t)hs[0]; dB[u * 32 * RPL] = (uint8_t)(hs[0] >> 16);
-								}
-								if(keepBottom && lane == 31) {
-									if(OFFDOM) bnd[j] = __byte_perm(botH, botF, 0x6420);
-									else reinterpret_cast<uint2 *>(bnd)[j] = make_uint2(botH, botF);
+								// byte 0 of every word is problem A's cell, byte 2 problem B's.  Under OFFDOM every lane stores at every
+								// step: a cell outside the lane's range lies before its first column (step < lane: read as "not stored") or
+								// right of the window (never read), and the steps of the last group past the block's end land in the
+								// stride's slack (dp_code_stride) or in the next block's first steps, which that block overwrites
+								if(OFFDOM || on) {
+									if(RPL == 2) {
+										const uint32_t w2 = __byte_perm(hs[0], hs[RPL - 1], 0x6240);
+										*reinterpret_cast<uint16_t *>(dA + u * 32 * RPL) = (uint16_t)w2;
+										*reinterpret_cast<uint16_t *>(dB + u * 32 * RPL) = (uint16_t)(w2 >> 16);
+									} else {
+										dA[u * 32 * RPL] = (uint8_t)hs[0]; dB[u * 32 * RPL] = (uint8_t)(hs[0] >> 16);
+									}
+									if(keepBottom && lane == 31 && on) {
+										if(OFFDOM) bnd[j] = __byte_perm(botH, botF, 0x6420);
+										else reinterpret_cast<uint2 *>(bnd)[j] = make_uint2(botH, botF);
+									}
 								}
 							} else {
 								botH = FLOORP; botF = FLOORP;                   // not started yet, or done with the window
