@@ -680,7 +680,7 @@ int bt2g_dp_extend(bt2g_ctx *ctx, const bt2g_reads *reads, const bt2g_dp_problem
 	if(maxLen > 512) { ctx->err = "reads longer than 512 are not supported by the DP kernel"; return -1; }
 	maxCol += 1;                              // local mode keeps one extra reference character
 	if(maxCol > 8192) { ctx->err = "DP window wider than 8192 columns"; return -1; }
-	DBuf dseq, dqual, doff, dprob, dcodes, dlast, dsumm, dcand, daln, dops, draw;
+	DBuf dseq, dqual, doff, dprob, dcodes, dlast, dsumm, dcand, daln, dops, draw, dctr;
 	int rc = uploadReads(ctx, reads, dseq, dqual, doff, true);
 	if(rc) return rc;
 	DpLaunch L;
@@ -696,6 +696,8 @@ int bt2g_dp_extend(bt2g_ctx *ctx, const bt2g_reads *reads, const bt2g_dp_problem
 	if(L.packed == 3) {
 		L.chunk = dp_chunk_problems(L.codeStride, n);
 		BT2G_CUDA_TRY(ctx, dcodes.alloc(L.chunk * L.codeStride));
+		BT2G_CUDA_TRY(ctx, dctr.alloc(4 * sizeof(uint32_t)));
+		L.taskCtr = dctr.as<uint32_t>();
 	} else {
 		BT2G_CUDA_TRY(ctx, dcodes.alloc(L.numSlots * L.codeStride * (L.packed ? 2 : 1)));
 	}

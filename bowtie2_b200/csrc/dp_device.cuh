@@ -11,8 +11,8 @@ static inline bool dp_packed_ok(const bt2g_scoring &sc, int64_t minMinsc, int ma
 
 // DpLaunch.packed: 0 = k_dp_e2e (32-bit, move codes), 1 = k_dp_e2e_x2 (s16x2, move codes),
 // 2 = k_dp_e2e_h (s16x2, H bytes: needs perfect - (minsc - bonus - 1) <= 127 for every problem),
-// 3 = the same split into k_dp_fill_h + k_dp_tail_h over chunks of DpLaunch.chunk problems
-//     (workspace: chunk * codeStride bytes).
+// 3 = the same split into k_dp_fill_h + k_dp_tail_h over chunks of a workspace of DpLaunch.chunk problems
+//     (chunk * codeStride bytes; chunks planned by dp_chunk_size).
 // `cap` (bt2g_ctx::dpModeCap, set by bt2g_set_dp_mode; initialised once from BT2G_DP_PACKED at bt2g_create) caps the mode.
 static inline int dp_kernel_mode(const bt2g_scoring &sc, int64_t minMinsc, int maxLen, int cap = 3) {
 	if(cap < 0 || cap > 3) cap = 3;
@@ -43,12 +43,23 @@ static inline uint64_t dp_code_stride(int maxCol, int maxLen, int mode) {
 	return ((steps * 32 * (uint64_t)R) + 255) & ~(uint64_t)255;   // planes of hb_index, 256 B aligned
 }
 
-// mode 3 workspace: as many problems per chunk as fit a byte budget (default 6 GiB; BT2G_DP_CHUNK_MB overrides)
+// mode 3 workspace: as many problems as fit a byte budget (default 6 GiB; BT2G_DP_CHUNK_MB overrides), at least 1024
 static inline uint64_t dp_chunk_problems(uint64_t codeStride, uint64_t nMax, uint64_t budget = 6ull << 30) {
 	if(const char *e = getenv("BT2G_DP_CHUNK_MB")) { uint64_t v = strtoull(e, nullptr, 10); if(v) budget = v << 20; }
 	uint64_t c = budget / (codeStride ? codeStride : 1);
 	if(c < 1024) c = 1024;
 	if(c > nMax) c = nMax;
+	return c ? c : 1;
+}
+
+// mode 3 chunk planning: a queue of n problems through a workspace (or half of one) of cap problems runs as k = ceil(n / cap)
+// chunks of equal size rather than full chunks and a small remainder, each rounded up to whole rounds of the fill (`round`:
+// the problems its resident warps hold at once) where cap allows: a chunk of 2.2 rounds takes as long as one of 3
+static inline uint64_t dp_chunk_size(uint64_t n, uint64_t cap, uint64_t round) {
+	if(cap < 1) cap = 1;
+	const uint64_t k = (n + cap - 1) / cap;
+	uint64_t c = k ? (n + k - 1) / k : cap;
+	if(round) { const uint64_t r = (c + round - 1) / round * round; if(r <= cap) c = r; }
 	return c ? c : 1;
 }
 
@@ -66,9 +77,13 @@ struct DpLaunch {
 	uint64_t        codeStride;
 	int             maxCol;
 	int             maxCands, maxAlns, maxOps;
-	uint64_t        chunk = 0;    // mode 3: problems per fill/tail chunk
+	uint64_t        chunk = 0;    // mode 3: problems the workspace holds (dp_chunk_problems); chunks are planned by dp_chunk_size
 	int             packed = 0;   // e2e: two problems per warp as s16x2 pairs (codes workspace: 2 * codeStride per slot)
-	cudaEvent_t    *tev = nullptr;  // optional timing marks (mode 3): one before the first fill, then one after every fill and every tail
+	uint32_t       *taskCtr = nullptr;  // mode 3 (required): 4 device words, the fill's and the tail's task counters of either half
+	cudaStream_t    st2 = nullptr;      // mode 3, optional: consecutive chunks alternate between the launch's stream and st2, each in
+	cudaEvent_t     evFork = nullptr, evJoin = nullptr;   // its own half of the workspace (st2 first waits for, then joins, the stream)
+	uint64_t       *nChunks = nullptr;  // mode 3, optional: chunks launched (a fill and a tail each)
+	cudaEvent_t    *tev = nullptr;  // optional timing marks (mode 3): before the fill, between fill and tail, after the tail of every chunk
 	int             tevCap = 0;
 	int            *tevN = nullptr;
 	uint32_t        zeroP = 0;    // always 0: a zero the compiler cannot see through, so that it stays in ONE register (a literal 0 as

@@ -781,14 +781,20 @@ __host__ __device__ __forceinline__ size_t dp_fill_smem_per_warp(int maxCol, boo
 
 template <bool B> struct DpBool { static constexpr bool value = B; };
 
+// the next task of a warp from a launch's task counter (lane 0 takes it, every lane gets it)
+__device__ __forceinline__ uint64_t dp_next_task(uint32_t *next, int lane) {
+	uint32_t t = 0;
+	if(lane == 0) t = atomicAdd(next, 1u);
+	return __shfl_sync(0xffffffffu, t, 0);
+}
+
 template <typename OFF, int R, bool OFFDOM>
-__global__ void __launch_bounds__(128, 8) k_dp_fill_h(DevIndex<OFF> ix, bt2g_scoring sc, DpLaunch L, uint64_t chunkStart, uint64_t chunkMax) {
+__global__ void __launch_bounds__(128, 8) k_dp_fill_h(DevIndex<OFF> ix, bt2g_scoring sc, DpLaunch L, uint64_t chunkStart, uint64_t chunkMax,
+                                                      uint32_t *next) {
 	constexpr int RPL = DP_BLOCK_RPL;
 	static_assert(RPL == 1 || RPL == 2, "stores are one byte or one u16 per lane and problem");
 	extern __shared__ uint8_t smem[];
 	const int warpInBlock = threadIdx.x >> 5, lane = threadIdx.x & 31;
-	const uint64_t slot = blockIdx.x * (uint64_t)(blockDim.x >> 5) + warpInBlock;
-	const uint64_t nSlots = (uint64_t)gridDim.x * (blockDim.x >> 5);
 	const uint64_t nAll = L.nDev ? (uint64_t)*L.nDev : L.n;
 	if(chunkStart >= nAll) return;
 	const uint64_t nProb = (nAll - chunkStart < chunkMax) ? nAll - chunkStart : chunkMax;   // problems of this chunk
@@ -818,7 +824,9 @@ __global__ void __launch_bounds__(128, 8) k_dp_fill_h(DevIndex<OFF> ix, bt2g_sco
 	const uint32_t FLOORP = OFFDOM ? L.zeroP : dpx_both(DPX_FLOOR);
 	const uint32_t nrdeP = dpx_both(-rdgape);
 
-	for(uint64_t pw = slot; pw < nPairs; pw += nSlots) {
+	// problem pairs are handed out by the chunk's counter (zeroed before the launch): a rectangle that costs more than the
+	// average holds up only its own warp, not the pairs a fixed stride would have queued behind it
+	for(uint64_t pw = dp_next_task(next, lane); pw < nPairs; pw = dp_next_task(next, lane)) {
 		uint64_t w[2] = {2 * pw, 2 * pw + 1};
 		bool live[2] = {true, w[1] < nProb};
 		if(!live[1]) w[1] = w[0];
@@ -1032,7 +1040,8 @@ struct DpHbBlocks {
 #define DP_TAIL_SMEM_PER_WARP(maxCol, R) (dp_smem_per_warp(maxCol) + DP_PROF_BYTES(R) + DP_BLK_MAX * sizeof(uint2))
 
 template <typename OFF, int R>
-__global__ void __launch_bounds__(256) k_dp_tail_h(DevIndex<OFF> ix, bt2g_scoring sc, DpLaunch L, uint64_t chunkStart, uint64_t chunkMax) {
+__global__ void __launch_bounds__(256) k_dp_tail_h(DevIndex<OFF> ix, bt2g_scoring sc, DpLaunch L, uint64_t chunkStart, uint64_t chunkMax,
+                                                   uint32_t *next) {
 	extern __shared__ uint8_t smem[];
 	const int warpInBlock = threadIdx.x >> 5, lane = threadIdx.x & 31;
 	const uint64_t nAll = L.nDev ? (uint64_t)*L.nDev : L.n;
@@ -1045,8 +1054,7 @@ __global__ void __launch_bounds__(256) k_dp_tail_h(DevIndex<OFF> ix, bt2g_scorin
 	uint8_t *prof = smem + (size_t)warpInBlock * perWarp + dp_smem_per_warp(L.maxCol);
 	uint2 *tab = reinterpret_cast<uint2 *>(prof + DP_PROF_BYTES(R));
 	const int bonus = sc.match_bonus;
-	const uint64_t nWarps = (uint64_t)gridDim.x * (blockDim.x >> 5);
-	for(uint64_t wl = blockIdx.x * (uint64_t)(blockDim.x >> 5) + warpInBlock; wl < nProb; wl += nWarps) {
+	for(uint64_t wl = dp_next_task(next, lane); wl < nProb; wl = dp_next_task(next, lane)) {
 		const uint64_t w = chunkStart + wl;
 		const bt2g_dp_problem p = L.probs[w];
 		const uint8_t *rs = L.seq + L.roff[p.read_idx], *rq = L.qual + L.roff[p.read_idx];
@@ -1346,10 +1354,14 @@ static unsigned dp_resident_grid(K kernel, int threads, size_t smem, uint64_t nu
 }
 
 template <typename OFF, int R>
-static void launch_dp_e2e_r(const DevIndex<OFF> &ix, const bt2g_scoring &sc, const DpLaunch &L, cudaStream_t st) {
+static int launch_dp_e2e_r(const DevIndex<OFF> &ix, const bt2g_scoring &sc, const DpLaunch &L, cudaStream_t st) {
 	const int warpsPerBlock = 4;
 	if(L.packed == 3) {
-		// split: chunks of L.chunk problems through fill then tail (workspace = L.chunk * codeStride bytes)
+		// split: chunks through fill then tail.  The workspace holds L.chunk problems; with L.st2 it is cut into two halves and
+		// chunk k runs in half k mod 2 on stream k mod 2 (st, L.st2), so that stream order alone makes the fill of chunk k wait
+		// for the tail of chunk k - 2 (the last user of its half) and its tail for its fill, while the fill of chunk k + 1
+		// overlaps them on the other stream.
+		if(!L.taskCtr) return -1;
 		int dev = 0, sms = 148; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
 		const size_t smF = (size_t)warpsPerBlock * dp_fill_smem_per_warp(L.maxCol, sc.match_bonus == 0);
 		const size_t smT = (size_t)8 * DP_TAIL_SMEM_PER_WARP(L.maxCol, R);
@@ -1359,14 +1371,30 @@ static void launch_dp_e2e_r(const DevIndex<OFF> &ix, const bt2g_scoring &sc, con
 		int nbF = 1, nbT = 1;
 		if(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nbF, kfill, warpsPerBlock * 32, smF) != cudaSuccess || nbF < 1) nbF = 1;
 		if(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nbT, k_dp_tail_h<OFF, R>, 256, smT) != cudaSuccess || nbT < 1) nbT = 1;
-		auto mark = [&]() { if(L.tev && L.tevN && *L.tevN < L.tevCap) cudaEventRecord(L.tev[(*L.tevN)++], st); };
-		mark();
-		for(uint64_t c0 = 0; c0 < L.n; c0 += L.chunk) {
-			kfill<<<(unsigned)(nbF * sms), warpsPerBlock * 32, smF, st>>>(ix, sc, L, c0, L.chunk);
-			mark();
-			k_dp_tail_h<OFF, R><<<(unsigned)(nbT * sms), 256, smT, st>>>(ix, sc, L, c0, L.chunk);
-			mark();
+		const int halves = (L.st2 && L.chunk >= 2) ? 2 : 1;
+		const uint64_t cap = L.chunk / halves;
+		const uint64_t c = dp_chunk_size(L.n, cap, 2ull * warpsPerBlock * nbF * sms);   // two problems per fill warp
+		cudaStream_t ss[2] = {st, L.st2};
+		if(halves == 2) { cudaEventRecord(L.evFork, st); cudaStreamWaitEvent(L.st2, L.evFork, 0); }
+		// timing marks: before the fill, between fill and tail, after the tail of every chunk
+		auto mark = [&](cudaStream_t s, int k) { cudaEventRecord(L.tev[*L.tevN + k], s); };
+		uint64_t k = 0;
+		for(uint64_t c0 = 0; c0 < L.n; c0 += c, k++) {
+			const int h = (int)(k % halves);
+			cudaStream_t s = ss[h];
+			DpLaunch Lc = L;
+			Lc.codes = L.codes + (uint64_t)h * cap * L.codeStride;
+			uint32_t *ctr = L.taskCtr + 2 * h;
+			cudaMemsetAsync(ctr, 0, 2 * sizeof(uint32_t), s);
+			const bool timed = L.tev && L.tevN && *L.tevN + 3 <= L.tevCap;
+			if(timed) mark(s, 0);
+			kfill<<<(unsigned)(nbF * sms), warpsPerBlock * 32, smF, s>>>(ix, sc, Lc, c0, c, ctr);
+			if(timed) mark(s, 1);
+			k_dp_tail_h<OFF, R><<<(unsigned)(nbT * sms), 256, smT, s>>>(ix, sc, Lc, c0, c, ctr + 1);
+			if(timed) { mark(s, 2); *L.tevN += 3; }
 		}
+		if(halves == 2 && k > 1) { cudaEventRecord(L.evJoin, L.st2); cudaStreamWaitEvent(st, L.evJoin, 0); }
+		if(L.nChunks) *L.nChunks = k;
 	} else if(L.packed == 2) {
 		const size_t smem = (size_t)warpsPerBlock * 2 * dp_smem_per_warp(L.maxCol);
 		if(smem > 48 * 1024) cudaFuncSetAttribute(k_dp_e2e_h<OFF, R>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -1383,6 +1411,7 @@ static void launch_dp_e2e_r(const DevIndex<OFF> &ix, const bt2g_scoring &sc, con
 		const unsigned grid = dp_resident_grid(k_dp_e2e<OFF, R>, warpsPerBlock * 32, smem, L.numSlots, warpsPerBlock);
 		k_dp_e2e<OFF, R><<<grid, warpsPerBlock * 32, smem, st>>>(ix, sc, L);
 	}
+	return 0;
 }
 
 // L.packed selects the two-problems-per-warp s16x2 kernel; the caller guarantees the score range
@@ -1391,16 +1420,15 @@ template <typename OFF>
 int launch_dp_e2e(const DevIndex<OFF> &ix, const bt2g_scoring &sc, const DpLaunch &L, int maxRdLen, cudaStream_t st) {
 	if(L.n == 0) return 0;
 	switch(dp_rows_per_lane(maxRdLen, L.packed)) {
-		case 4: launch_dp_e2e_r<OFF, 4>(ix, sc, L, st); break;
-		case 5: launch_dp_e2e_r<OFF, 5>(ix, sc, L, st); break;
-		case 6: launch_dp_e2e_r<OFF, 6>(ix, sc, L, st); break;
-		case 8: launch_dp_e2e_r<OFF, 8>(ix, sc, L, st); break;
-		case 10: launch_dp_e2e_r<OFF, 10>(ix, sc, L, st); break;
-		case 12: launch_dp_e2e_r<OFF, 12>(ix, sc, L, st); break;
-		case 16: launch_dp_e2e_r<OFF, 16>(ix, sc, L, st); break;
+		case 4: return launch_dp_e2e_r<OFF, 4>(ix, sc, L, st);
+		case 5: return launch_dp_e2e_r<OFF, 5>(ix, sc, L, st);
+		case 6: return launch_dp_e2e_r<OFF, 6>(ix, sc, L, st);
+		case 8: return launch_dp_e2e_r<OFF, 8>(ix, sc, L, st);
+		case 10: return launch_dp_e2e_r<OFF, 10>(ix, sc, L, st);
+		case 12: return launch_dp_e2e_r<OFF, 12>(ix, sc, L, st);
+		case 16: return launch_dp_e2e_r<OFF, 16>(ix, sc, L, st);
 		default: return -1;
 	}
-	return 0;
 }
 template int launch_dp_e2e<uint32_t>(const DevIndex<uint32_t> &, const bt2g_scoring &, const DpLaunch &, int, cudaStream_t);
 template int launch_dp_e2e<uint64_t>(const DevIndex<uint64_t> &, const bt2g_scoring &, const DpLaunch &, int, cudaStream_t);

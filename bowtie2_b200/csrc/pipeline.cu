@@ -45,7 +45,7 @@ struct PipeBufs {
 	uint32_t *nRows, *rowBase, *rowCnt;
 	uint64_t *tidx, *textoff, *tlen; uint8_t *rflags;   // resolve
 	bt2g_dp_problem *probs; uint32_t *nProb; int32_t *readProb; int32_t *readNProb;
-	uint8_t *codes; int32_t *lastH; uint64_t *rawKeys;
+	uint8_t *codes; int32_t *lastH; uint64_t *rawKeys; uint32_t *dpTasks;   // dpTasks: task counters of the split DP kernels
 	bt2g_dp_summary *summ; bt2g_dp_cand *cands; bt2g_dp_aln *alns; uint8_t *ops;
 	bt2g_read_result *res; uint8_t *resOps;
 	unsigned long long *counters;             // [4]: sweep sides, seed sides, resolve sides, dp cells
@@ -436,7 +436,7 @@ static int runStages(bt2g_pipeline *p, const uint8_t *seq, const uint8_t *qual, 
 	L.seq = seq; L.qual = qual; L.roff = roff; L.probs = b.probs; L.n = p->maxProbs; L.nDev = b.nProb;
 	L.rawKeys = b.rawKeys; L.maxRaw = b.rawKeys ? PIPE_MAX_RAW : 0;
 	L.numSlots = p->numSlots; L.codes = b.codes; L.lastH = b.lastH; L.codeStride = p->codeStride; L.maxCol = p->maxCol;
-	L.maxCands = q.max_cands; L.maxAlns = q.max_alns; L.maxOps = q.max_ops; L.packed = p->packed; L.chunk = p->dpChunk;
+	L.maxCands = q.max_cands; L.maxAlns = q.max_alns; L.maxOps = q.max_ops; L.packed = p->packed; L.chunk = p->dpChunk; L.taskCtr = b.dpTasks;
 	L.summ = b.summ; L.cands = b.cands; L.alns = b.alns; L.ops = b.ops;
 	mark(6);
 	const int drc = p->sc.local ? launch_dp_local<OFF>(ix, p->sc, L, q.max_len, st) : launch_dp_e2e<OFF>(ix, p->sc, L, q.max_len, st);
@@ -471,7 +471,7 @@ static int runPairTail(bt2g_pipeline *p, const uint8_t *seq, const uint8_t *qual
 	L.seq = seq; L.qual = qual; L.roff = roff; L.probs = b.mProbs; L.n = p->maxReads; L.nDev = b.nMateProb;
 	L.rawKeys = nullptr; L.maxRaw = 0;
 	L.numSlots = p->numSlots; L.codes = b.codes; L.lastH = nullptr; L.codeStride = p->mateCodeStride; L.maxCol = p->mateMaxCol;
-	L.maxCands = q.max_cands; L.maxAlns = q.max_alns; L.maxOps = q.max_ops; L.packed = p->packed; L.chunk = p->mateChunk;
+	L.maxCands = q.max_cands; L.maxAlns = q.max_alns; L.maxOps = q.max_ops; L.packed = p->packed; L.chunk = p->mateChunk; L.taskCtr = b.dpTasks;
 	L.summ = b.mSumm; L.cands = b.mCands; L.alns = b.mAlns; L.ops = b.mOps;
 	if(launch_dp_e2e<OFF>(ix, p->sc, L, q.max_len, st)) { ctx->err = "pipeline: mate DP launch rejected"; return -1; }
 	cudaEventRecord(p->pev[2], st);
@@ -536,7 +536,7 @@ int bt2g_pipeline_create(bt2g_ctx *ctx, const bt2g_pipeline_params *prm, uint64_
 	rc |= pipeAlloc(p, b.summ, nprobMax); rc |= pipeAlloc(p, b.cands, nprobMax * prm->max_cands);
 	rc |= pipeAlloc(p, b.alns, nprobMax * prm->max_alns); rc |= pipeAlloc(p, b.ops, nprobMax * prm->max_alns * (uint64_t)prm->max_ops);
 	rc |= pipeAlloc(p, b.res, n); rc |= pipeAlloc(p, b.resOps, n * (uint64_t)prm->max_ops);
-	rc |= pipeAlloc(p, b.counters, 4);
+	rc |= pipeAlloc(p, b.counters, 4); rc |= pipeAlloc(p, b.dpTasks, 4);
 	rc |= pipeAlloc(p, b.probTlen, nprobMax); rc |= pipeAlloc(p, b.resTlen, n);
 	if(rc) { bt2g_pipeline_destroy(p); return -2; }
 	cudaError_t e = cudaSuccess;

@@ -37,7 +37,7 @@ namespace {
 using namespace xe;
 
 #define XE_MM_MAXHITS 16
-#define XE_TEV 96                    // timing marks per DP queue and wave (fill / tail split; chunks beyond that go unsplit)
+#define XE_TEV 192                   // timing marks per DP queue and wave: 3 per chunk (fill / tail split; chunks beyond 64 go untimed)
 
 struct XQueues {                     // per wave, reset before k_xe_step
 	uint32_t nDpA, nDpM, nMm, nSeed, nDone, nFallback, nActive, pad1;
@@ -248,7 +248,7 @@ __global__ void __launch_bounds__(128) k_xe_report(XParams P, const XUnit *units
 }
 
 struct DpWork {                       // workspace of one DP queue (anchor rectangles / mate rectangles)
-	DpOut o{}; uint8_t *codes = nullptr; int32_t *lastH = nullptr; uint64_t *rawKeys = nullptr;
+	DpOut o{}; uint8_t *codes = nullptr; int32_t *lastH = nullptr; uint64_t *rawKeys = nullptr; uint32_t *tasks = nullptr;
 	int maxCol = 0, packed = 0, maxRaw = 0; uint64_t codeStride = 0, chunk = 0, numSlots = 0;
 };
 
@@ -283,6 +283,8 @@ struct bt2g_xengine {
 	float stageMs[12] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};   // [8], [9]: DP fill / DP tail kernels of both queues (split of [4] + [5])
 	cudaEvent_t tev[2][XE_TEV]; int tevN[2] = {0, 0};
 	cudaEvent_t evJoin = nullptr; int dpSideBySide = 1;   // BT2G_XE_DP_SERIAL=1 turns the side-by-side DP launches of small waves off
+	cudaEvent_t evFork = nullptr;      // the split DP's second stream waits for the first (DpLaunch::st2)
+	cudaStream_t streamDp = nullptr;   // normal priority: the split DP's odd chunks in full waves (DpLaunch::st2)
 	uint64_t launches = 0;             // kernels of this library launched by the last batch
 	// -k / -a engines (bt2g_xengine_create_k): the dense entry arrays of the last batch (d.res / resOps / pairs stay unallocated)
 	uint32_t maxPer = 0;
@@ -310,8 +312,11 @@ int setupDp(bt2g_xengine *e, DpWork &w, int maxCol, uint64_t cap, int maxCands, 
 	w.codeStride = dp_code_stride(w.maxCol, e->maxLen, w.packed);
 	w.numSlots = (uint64_t)e->sms * 24;
 	int rc = 0;
-	// (3 GiB of H-byte workspace per queue: a chunk still holds tens of thousands of problems, and several engines fit one GPU)
-	if(w.packed == 3) { w.chunk = dp_chunk_problems(w.codeStride, cap, 3ull << 30); rc |= xalloc(e, w.codes, w.chunk * w.codeStride); }
+	// (3 GiB of H-byte workspace per queue: each half still holds a resident round of the fill, and several engines fit one GPU)
+	if(w.packed == 3) {
+		w.chunk = dp_chunk_problems(w.codeStride, cap, 3ull << 30);
+		rc |= xalloc(e, w.codes, w.chunk * w.codeStride); rc |= xalloc(e, w.tasks, 4);
+	}
 	else rc |= xalloc(e, w.codes, w.numSlots * w.codeStride * (w.packed ? 2 : 1));
 	rc |= xalloc(e, w.lastH, w.numSlots * (uint64_t)w.maxCol);
 	w.maxRaw = maxCands * 4 < 1024 ? 1024 : maxCands * 4;
@@ -322,19 +327,23 @@ int setupDp(bt2g_xengine *e, DpWork &w, int maxCol, uint64_t cap, int maxCands, 
 	return rc;
 }
 
+// st2 (optional): the split DP alternates its chunks between st and st2 (DpLaunch::st2)
 template <typename OFF>
-int launchDp(bt2g_xengine *e, const DpWork &w, uint64_t n, cudaStream_t st) {
+int launchDp(bt2g_xengine *e, const DpWork &w, uint64_t n, cudaStream_t st, cudaStream_t st2) {
 	if(n == 0) return 0;
 	DpLaunch L;
 	L.seq = e->d.seq; L.qual = e->d.qual; L.roff = e->d.roff; L.probs = w.o.probs; L.n = n; L.nDev = nullptr;
 	L.numSlots = w.numSlots; L.codes = w.codes; L.lastH = w.lastH; L.rawKeys = w.rawKeys; L.maxRaw = w.rawKeys ? w.maxRaw : 0;
 	L.codeStride = w.codeStride; L.maxCol = w.maxCol; L.maxCands = w.o.maxCands; L.maxAlns = w.o.maxAlns; L.maxOps = w.o.maxOps;
-	L.chunk = w.chunk; L.packed = w.packed;
+	L.chunk = w.chunk; L.packed = w.packed; L.taskCtr = w.tasks;
+	L.st2 = st2; L.evFork = e->evFork; L.evJoin = e->evJoin;
+	uint64_t chunks = 0; L.nChunks = &chunks;
 	{ const int qi = &w == &e->M ? 1 : 0; e->tevN[qi] = 0; L.tev = e->tev[qi]; L.tevCap = XE_TEV; L.tevN = &e->tevN[qi]; }
 	L.summ = w.o.summ; L.cands = w.o.cands; L.alns = w.o.alns; L.ops = w.o.ops;
 	const DevIndex<OFF> ix = bt2g_dev_index<OFF>(e->ctx);
-	e->launches += (!e->sc.local && w.packed == 3) ? 2 * ((n + w.chunk - 1) / w.chunk) : 1;
-	return e->sc.local ? launch_dp_local<OFF>(ix, e->sc, L, e->maxLen, st) : launch_dp_e2e<OFF>(ix, e->sc, L, e->maxLen, st);
+	const int rc = e->sc.local ? launch_dp_local<OFF>(ix, e->sc, L, e->maxLen, st) : launch_dp_e2e<OFF>(ix, e->sc, L, e->maxLen, st);
+	e->launches += (!e->sc.local && w.packed == 3) ? 2 * chunks : 1;
+	return rc;
 }
 
 // the waves of one batch whose reads are in device memory (e->d.seq / qual / roff set)
@@ -387,8 +396,11 @@ int runBatch(bt2g_xengine *e, uint64_t nReads, const char *dNames, uint32_t name
 		BT2G_CUDA_TRY(ctx, cudaStreamSynchronize(st));
 		// everything recorded before this synchronisation has completed: the primitives of the previous wave and this step
 		if(wave == 0) lap(7, 0, 0); else { lap(2, 3, 2); lap(3, 4, 3); lap(4, 5, 4); lap(5, 0, 5); }
-		for(int qi = 0; qi < 2; qi++) {                   // fill / tail split of the DP launches of the previous wave
-			for(int k = 0; k + 1 < e->tevN[qi]; k++) { float ms = 0.f; if(cudaEventElapsedTime(&ms, e->tev[qi][k], e->tev[qi][k + 1]) == cudaSuccess) e->stageMs[8 + (k & 1)] += ms; }
+		for(int qi = 0; qi < 2; qi++) {                   // fill / tail split of the DP launches of the previous wave: per chunk, the
+			for(int k = 0; k + 1 < e->tevN[qi]; k++) {    // marks before the fill, between fill and tail and after the tail (one stream)
+				if(k % 3 == 2) continue;
+				float ms = 0.f; if(cudaEventElapsedTime(&ms, e->tev[qi][k], e->tev[qi][k + 1]) == cudaSuccess) e->stageMs[8 + k % 3] += ms;
+			}
 			e->tevN[qi] = 0;
 		}
 		lap(0, 1, 1);
@@ -422,9 +434,13 @@ int runBatch(bt2g_xengine *e, uint64_t nReads, const char *dNames, uint32_t name
 		// side by side on the engine's two streams instead of one after the other (everything before this point has completed)
 		const bool sideBySide = e->ownStreams && e->dpSideBySide && q.nDpA && q.nDpM && (uint64_t)(q.nDpA + q.nDpM) * 16 <= (uint64_t)e->sms * 2048;
 		cudaStream_t stM = sideBySide ? (st == e->stream ? e->streamHi : e->stream) : st;
-		if(launchDp<OFF>(e, e->A, q.nDpA, st)) { ctx->err = "xengine: DP launch rejected"; return -1; }
+		// each queue's chunks alternate between two of the engine's streams, so that one chunk's fill overlaps the previous
+		// chunk's tail (DpLaunch::st2).  In the full waves the second one is streamDp, of normal priority like e->stream: on
+		// streamHi every other chunk's blocks would be scheduled ahead of the other engines' pending blocks, which measured slower
+		cudaStream_t st2 = (e->ownStreams && !sideBySide) ? (st == e->stream ? e->streamDp : e->stream) : nullptr;
+		if(launchDp<OFF>(e, e->A, q.nDpA, st, st2)) { ctx->err = "xengine: DP launch rejected"; return -1; }
 		cudaEventRecord(ev[5], st);
-		if(launchDp<OFF>(e, e->M, q.nDpM, stM)) { ctx->err = "xengine: DP launch rejected"; return -1; }
+		if(launchDp<OFF>(e, e->M, q.nDpM, stM, st2)) { ctx->err = "xengine: DP launch rejected"; return -1; }
 		if(sideBySide) { cudaEventRecord(e->evJoin, stM); cudaStreamWaitEvent(st, e->evJoin, 0); }
 		cudaEventRecord(ev[0], st);
 		BT2G_CUDA_TRY(ctx, cudaGetLastError());
@@ -529,8 +545,10 @@ static int createEngine(bt2g_ctx *ctx, const bt2g_policy_params *pp, uint64_t ma
 		for(int k = 0; k < 8 && err == cudaSuccess; k++) err = cudaEventCreate(&e->ev[k]);
 		for(int k = 0; k < 2 * XE_TEV && err == cudaSuccess; k++) err = cudaEventCreate(&e->tev[k / XE_TEV][k % XE_TEV]);
 		if(err == cudaSuccess) err = cudaEventCreateWithFlags(&e->evJoin, cudaEventDisableTiming);
+		if(err == cudaSuccess) err = cudaEventCreateWithFlags(&e->evFork, cudaEventDisableTiming);
 		if(err == cudaSuccess) err = cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking);
 		if(err == cudaSuccess) { int lo = 0, hi = 0; cudaDeviceGetStreamPriorityRange(&lo, &hi); err = cudaStreamCreateWithPriority(&e->streamHi, cudaStreamNonBlocking, hi); }
+		if(err == cudaSuccess) err = cudaStreamCreateWithFlags(&e->streamDp, cudaStreamNonBlocking);
 	}
 	if(rc || err != cudaSuccess) {
 		if(err != cudaSuccess) ctx->err = std::string("xengine setup: ") + cudaGetErrorString(err);
@@ -573,8 +591,10 @@ void bt2g_xengine_destroy(bt2g_xengine *e) {
 	for(int k = 0; k < 8; k++) if(e->ev[k]) cudaEventDestroy(e->ev[k]);
 	for(int k = 0; k < 2 * XE_TEV; k++) if(e->tev[k / XE_TEV][k % XE_TEV]) cudaEventDestroy(e->tev[k / XE_TEV][k % XE_TEV]);
 	if(e->evJoin) cudaEventDestroy(e->evJoin);
+	if(e->evFork) cudaEventDestroy(e->evFork);
 	if(e->stream) cudaStreamDestroy(e->stream);
 	if(e->streamHi) cudaStreamDestroy(e->streamHi);
+	if(e->streamDp) cudaStreamDestroy(e->streamDp);
 	delete e;
 }
 
