@@ -679,7 +679,9 @@ int bt2g_dp_extend(bt2g_ctx *ctx, const bt2g_reads *reads, const bt2g_dp_problem
 	}
 	if(maxLen > 512) { ctx->err = "reads longer than 512 are not supported by the DP kernel"; return -1; }
 	maxCol += 1;                              // local mode keeps one extra reference character
-	if(maxCol > 8192) { ctx->err = "DP window wider than 8192 columns"; return -1; }
+	// (columns are 16-bit in the kernels; the mate windows of -X 8000 are about 8200 wide, and the kernels take fewer warps per
+	// block as windows widen)
+	if(maxCol > 16384) { ctx->err = "DP window wider than 16384 columns"; return -1; }
 	DBuf dseq, dqual, doff, dprob, dcodes, dlast, dsumm, dcand, daln, dops, draw, dctr;
 	int rc = uploadReads(ctx, reads, dseq, dqual, doff, true);
 	if(rc) return rc;

@@ -1353,9 +1353,27 @@ static unsigned dp_resident_grid(K kernel, int threads, size_t smem, uint64_t nu
 	return (unsigned)(g < cap ? g : cap);
 }
 
+// warps per block of a DP kernel whose warps take perWarp bytes of dynamic shared memory each: `want`, or fewer when a block of
+// `want` warps would pass the device's opt-in limit per block (wide windows: 4 warps of k_dp_e2e_x2 pass 227 KB from about 4100
+// columns).  Sets *smem and lets the kernel take it; 0 when not even one warp fits or the kernel's limit cannot be raised.
+template <typename K>
+static int dp_block_warps(K kernel, size_t perWarp, int want, size_t *smem) {
+	int dev = 0, optin = 48 * 1024;
+	cudaGetDevice(&dev);
+	if(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) != cudaSuccess) return 0;
+	cudaFuncAttributes fa;
+	if(cudaFuncGetAttributes(&fa, kernel) != cudaSuccess) return 0;
+	const size_t room = (size_t)optin > fa.sharedSizeBytes ? (size_t)optin - fa.sharedSizeBytes : 0;
+	int w = want;
+	while(w > 1 && (size_t)w * perWarp > room) w--;
+	if((size_t)w * perWarp > room) return 0;
+	*smem = (size_t)w * perWarp;
+	if(*smem > 48 * 1024 && cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)*smem) != cudaSuccess) return 0;
+	return w;
+}
+
 template <typename OFF, int R>
 static int launch_dp_e2e_r(const DevIndex<OFF> &ix, const bt2g_scoring &sc, const DpLaunch &L, cudaStream_t st) {
-	const int warpsPerBlock = 4;
 	if(L.packed == 3) {
 		// split: chunks through fill then tail.  The workspace holds L.chunk problems; with L.st2 it is cut into two halves and
 		// chunk k runs in half k mod 2 on stream k mod 2 (st, L.st2), so that stream order alone makes the fill of chunk k wait
@@ -1363,17 +1381,17 @@ static int launch_dp_e2e_r(const DevIndex<OFF> &ix, const bt2g_scoring &sc, cons
 		// overlaps them on the other stream.
 		if(!L.taskCtr) return -1;
 		int dev = 0, sms = 148; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-		const size_t smF = (size_t)warpsPerBlock * dp_fill_smem_per_warp(L.maxCol, sc.match_bonus == 0);
-		const size_t smT = (size_t)8 * DP_TAIL_SMEM_PER_WARP(L.maxCol, R);
+		size_t smF = 0, smT = 0;
 		auto kfill = sc.match_bonus == 0 ? k_dp_fill_h<OFF, R, true> : k_dp_fill_h<OFF, R, false>;
-		if(smF > 48 * 1024) cudaFuncSetAttribute(kfill, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smF);
-		if(smT > 48 * 1024) cudaFuncSetAttribute(k_dp_tail_h<OFF, R>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smT);
+		const int wF = dp_block_warps(kfill, dp_fill_smem_per_warp(L.maxCol, sc.match_bonus == 0), 4, &smF);
+		const int wT = dp_block_warps(k_dp_tail_h<OFF, R>, DP_TAIL_SMEM_PER_WARP(L.maxCol, R), 8, &smT);
+		if(!wF || !wT) return -1;
 		int nbF = 1, nbT = 1;
-		if(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nbF, kfill, warpsPerBlock * 32, smF) != cudaSuccess || nbF < 1) nbF = 1;
-		if(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nbT, k_dp_tail_h<OFF, R>, 256, smT) != cudaSuccess || nbT < 1) nbT = 1;
+		if(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nbF, kfill, wF * 32, smF) != cudaSuccess || nbF < 1) nbF = 1;
+		if(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nbT, k_dp_tail_h<OFF, R>, wT * 32, smT) != cudaSuccess || nbT < 1) nbT = 1;
 		const int halves = (L.st2 && L.chunk >= 2) ? 2 : 1;
 		const uint64_t cap = L.chunk / halves;
-		const uint64_t c = dp_chunk_size(L.n, cap, 2ull * warpsPerBlock * nbF * sms);   // two problems per fill warp
+		const uint64_t c = dp_chunk_size(L.n, cap, 2ull * wF * nbF * sms);   // two problems per fill warp
 		cudaStream_t ss[2] = {st, L.st2};
 		if(halves == 2) { cudaEventRecord(L.evFork, st); cudaStreamWaitEvent(L.st2, L.evFork, 0); }
 		// timing marks: before the fill, between fill and tail, after the tail of every chunk
@@ -1388,28 +1406,31 @@ static int launch_dp_e2e_r(const DevIndex<OFF> &ix, const bt2g_scoring &sc, cons
 			cudaMemsetAsync(ctr, 0, 2 * sizeof(uint32_t), s);
 			const bool timed = L.tev && L.tevN && *L.tevN + 3 <= L.tevCap;
 			if(timed) mark(s, 0);
-			kfill<<<(unsigned)(nbF * sms), warpsPerBlock * 32, smF, s>>>(ix, sc, Lc, c0, c, ctr);
+			kfill<<<(unsigned)(nbF * sms), wF * 32, smF, s>>>(ix, sc, Lc, c0, c, ctr);
 			if(timed) mark(s, 1);
-			k_dp_tail_h<OFF, R><<<(unsigned)(nbT * sms), 256, smT, s>>>(ix, sc, Lc, c0, c, ctr + 1);
+			k_dp_tail_h<OFF, R><<<(unsigned)(nbT * sms), wT * 32, smT, s>>>(ix, sc, Lc, c0, c, ctr + 1);
 			if(timed) { mark(s, 2); *L.tevN += 3; }
 		}
 		if(halves == 2 && k > 1) { cudaEventRecord(L.evJoin, L.st2); cudaStreamWaitEvent(st, L.evJoin, 0); }
 		if(L.nChunks) *L.nChunks = k;
 	} else if(L.packed == 2) {
-		const size_t smem = (size_t)warpsPerBlock * 2 * dp_smem_per_warp(L.maxCol);
-		if(smem > 48 * 1024) cudaFuncSetAttribute(k_dp_e2e_h<OFF, R>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-		const unsigned grid = dp_resident_grid(k_dp_e2e_h<OFF, R>, warpsPerBlock * 32, smem, L.numSlots, warpsPerBlock);
-		k_dp_e2e_h<OFF, R><<<grid, warpsPerBlock * 32, smem, st>>>(ix, sc, L);
+		size_t smem = 0;
+		const int w = dp_block_warps(k_dp_e2e_h<OFF, R>, 2 * dp_smem_per_warp(L.maxCol), 4, &smem);
+		if(!w) return -1;
+		const unsigned grid = dp_resident_grid(k_dp_e2e_h<OFF, R>, w * 32, smem, L.numSlots, w);
+		k_dp_e2e_h<OFF, R><<<grid, w * 32, smem, st>>>(ix, sc, L);
 	} else if(L.packed) {
-		const size_t smem = (size_t)warpsPerBlock * 2 * dp_smem_per_warp(L.maxCol);
-		if(smem > 48 * 1024) cudaFuncSetAttribute(k_dp_e2e_x2<OFF, R>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-		const unsigned grid = dp_resident_grid(k_dp_e2e_x2<OFF, R>, warpsPerBlock * 32, smem, L.numSlots, warpsPerBlock);
-		k_dp_e2e_x2<OFF, R><<<grid, warpsPerBlock * 32, smem, st>>>(ix, sc, L);
+		size_t smem = 0;
+		const int w = dp_block_warps(k_dp_e2e_x2<OFF, R>, 2 * dp_smem_per_warp(L.maxCol), 4, &smem);
+		if(!w) return -1;
+		const unsigned grid = dp_resident_grid(k_dp_e2e_x2<OFF, R>, w * 32, smem, L.numSlots, w);
+		k_dp_e2e_x2<OFF, R><<<grid, w * 32, smem, st>>>(ix, sc, L);
 	} else {
-		const size_t smem = (size_t)warpsPerBlock * dp_smem_per_warp(L.maxCol);
-		if(smem > 48 * 1024) cudaFuncSetAttribute(k_dp_e2e<OFF, R>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-		const unsigned grid = dp_resident_grid(k_dp_e2e<OFF, R>, warpsPerBlock * 32, smem, L.numSlots, warpsPerBlock);
-		k_dp_e2e<OFF, R><<<grid, warpsPerBlock * 32, smem, st>>>(ix, sc, L);
+		size_t smem = 0;
+		const int w = dp_block_warps(k_dp_e2e<OFF, R>, dp_smem_per_warp(L.maxCol), 4, &smem);
+		if(!w) return -1;
+		const unsigned grid = dp_resident_grid(k_dp_e2e<OFF, R>, w * 32, smem, L.numSlots, w);
+		k_dp_e2e<OFF, R><<<grid, w * 32, smem, st>>>(ix, sc, L);
 	}
 	return 0;
 }
@@ -1599,23 +1620,17 @@ __global__ void __launch_bounds__(128) k_dp_local(DevIndex<OFF> ix, bt2g_scoring
 template <typename OFF>
 int launch_dp_local(const DevIndex<OFF> &ix, const bt2g_scoring &sc, const DpLaunch &L, int maxRdLen, cudaStream_t st) {
 	if(L.n == 0) return 0;
-	const int warpsPerBlock = 4;
-	const size_t perWarp = dp_smem_per_warp(L.maxCol);
-	size_t smem = (size_t)warpsPerBlock * perWarp;
-	unsigned grid = (unsigned)(L.numSlots / warpsPerBlock);
-	if(maxRdLen <= 128) {
-		if(smem > 48 * 1024) cudaFuncSetAttribute(k_dp_local<OFF, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-		k_dp_local<OFF, 4><<<grid, warpsPerBlock * 32, smem, st>>>(ix, sc, L);
-	} else if(maxRdLen <= 256) {
-		if(smem > 48 * 1024) cudaFuncSetAttribute(k_dp_local<OFF, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-		k_dp_local<OFF, 8><<<grid, warpsPerBlock * 32, smem, st>>>(ix, sc, L);
-	} else if(maxRdLen <= 512) {
-		if(smem > 48 * 1024) cudaFuncSetAttribute(k_dp_local<OFF, 16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-		k_dp_local<OFF, 16><<<grid, warpsPerBlock * 32, smem, st>>>(ix, sc, L);
-	} else {
-		return -1;
-	}
-	return 0;
+	auto launch = [&](auto kernel) {
+		size_t smem = 0;
+		const int w = dp_block_warps(kernel, dp_smem_per_warp(L.maxCol), 4, &smem);
+		if(!w) return -1;
+		kernel<<<(unsigned)(L.numSlots / w), w * 32, smem, st>>>(ix, sc, L);
+		return 0;
+	};
+	if(maxRdLen <= 128) return launch(k_dp_local<OFF, 4>);
+	if(maxRdLen <= 256) return launch(k_dp_local<OFF, 8>);
+	if(maxRdLen <= 512) return launch(k_dp_local<OFF, 16>);
+	return -1;
 }
 template int launch_dp_local<uint32_t>(const DevIndex<uint32_t> &, const bt2g_scoring &, const DpLaunch &, int, cudaStream_t);
 template int launch_dp_local<uint64_t>(const DevIndex<uint64_t> &, const bt2g_scoring &, const DpLaunch &, int, cudaStream_t);

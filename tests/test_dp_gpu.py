@@ -34,15 +34,16 @@ def _problems(genome, reads, truth, sc, jitter_rng, minsc_bump=0):
     return np.array(probs, dtype=DP_PROBLEM), meta
 
 
-def _check(gpu, R, genome, reads, quals, probs, meta, local=False):
+def _check(gpu, R, genome, reads, quals, probs, meta, local=False, max_cands=None):
     batch = ReadBatch.from_list(reads, quals)
-    summ, cands, alns, ops = gpu.dp_extend(batch, probs, max_cands=8192 if local else 256, max_alns=24 if local else 8,
+    summ, cands, alns, ops = gpu.dp_extend(batch, probs, max_cands=max_cands or (8192 if local else 256), max_alns=24 if local else 8,
                                            max_ops=int(batch.lengths().max()) + 80)
     nfound = naln = ngap = 0
     for k, pr in enumerate(probs):
         tlen, rect, minsc = meta[k]
         i = int(pr["read_idx"])
-        want = ref_dp(R, local, reads[i], quals[i], int(pr["fw"]), int(pr["tidx"]), tlen, rect, minsc, max_cands=16384, max_alns=64, max_edits=16384)
+        want = ref_dp(R, local, reads[i], quals[i], int(pr["fw"]), int(pr["tidx"]), tlen, rect, minsc, max_cands=max(16384, max_cands or 0),
+                      max_alns=64, max_edits=16384)
         s = summ[k]
         assert s["flags"] == 0, (k, s)
         assert bool(s["found"]) == bool(want["found"]), (k, s, want["found"], want["best"])
