@@ -187,7 +187,9 @@ __global__ void __launch_bounds__(256) k_seed_search3(DevIndex<OFF> ix, const ui
                                                       int nofw, int norc, const int32_t *interval, const int32_t *offset,
                                                       uint64_t *out, int32_t *nseedsOut, unsigned long long *next,
                                                       unsigned long long *cnt, const uint8_t *actv) {
-	// actv != nullptr: only reads with actv[rd] != 0 are searched (their output slots are rewritten; the others stay untouched)
+	// actv != nullptr: only reads with actv[rd] != 0 are searched (their output slots are rewritten; the others stay untouched);
+	// bits 1 and 2 of actv[rd] skip that read's forward / reverse-complement seeds as nofw / norc skip every read's (the device
+	// engine's per-mate --nofw / --norc, SeedAligner::instantiateSeeds)
 	constexpr uint32_t BL = SideGeom<OFF>::BWT_LEN;
 	const unsigned FULL = 0xffffffffu;
 	const int lane = threadIdx.x & 31;
@@ -195,7 +197,7 @@ __global__ void __launch_bounds__(256) k_seed_search3(DevIndex<OFF> ix, const ui
 	const DevEbwt<OFF> &fw = ix.fw;
 	const DevEbwt<OFF> &bw = ix.bw;
 	const int ftabLen = fw.ftabChars;
-	bool haveTask = false, exhausted = false, active = false;
+	bool haveTask = false, exhausted = false, active = false, skip = false;
 	uint64_t topf = 0, botf = 0, topb = 0, botb = 0, bits = 0, wb = 0;
 	uint64_t *o = nullptr, *obase = nullptr;
 	int sl = 0, step = 0, k = 0, nseeds = 0, per = 1, off0 = 0, len = 0, strand = 0;
@@ -214,6 +216,7 @@ __global__ void __launch_bounds__(256) k_seed_search3(DevIndex<OFF> ix, const ui
 				else {
 					const uint64_t rd = t >> 1;
 					strand = (int)(t & 1);
+					skip = (strand == 0 ? nofw : norc) || (actv && ((actv[rd] >> (1 + strand)) & 1));
 					const uint64_t r0 = roff[rd];
 					len = (int)(roff[rd + 1] - r0);
 					per = interval[rd]; off0 = offset[rd];
@@ -239,7 +242,7 @@ __global__ void __launch_bounds__(256) k_seed_search3(DevIndex<OFF> ix, const ui
 				reinterpret_cast<uint4 *>(o)[0] = make_uint4(0, 0, 0, 0);
 				reinterpret_cast<uint4 *>(o)[1] = make_uint4(0, 0, 0, 0);
 				const int depth = k * per + off0;
-				bool ok = k < nseeds && !((strand == 0 && nofw) || (strand == 1 && norc)) && depth + sl <= len && sl >= 1;
+				bool ok = k < nseeds && !skip && depth + sl <= len && sl >= 1;
 				if(ok) {
 					const int w = depth >> 5, sh = depth & 31;
 					const bool two = sh + sl > 32;

@@ -191,7 +191,8 @@ __global__ void __launch_bounds__(128, MINB) k_xe_step(DevIndex<OFF> ix, bt2g_sc
 			u.dpSlot = (int32_t)slot;
 			break; }
 		case XR_SEED:
-			d.seedActive[u.rqRead] = 1; d.seedInterval[u.rqRead] = u.rqInterval; d.seedOffset[u.rqRead] = u.rqOffset;
+			d.seedActive[u.rqRead] = (uint8_t)(1 | (u.rqNofw ? 2 : 0) | (u.rqNorc ? 4 : 0));     // (the mate's --nofw / --norc)
+			d.seedInterval[u.rqRead] = u.rqInterval; d.seedOffset[u.rqRead] = u.rqOffset;
 			agg_inc(&d.q->nSeed);
 			break;
 		case XR_DONE: {
@@ -321,7 +322,7 @@ int setupDp(bt2g_xengine *e, DpWork &w, int maxCol, uint64_t cap, int maxCands, 
 	rc |= xalloc(e, w.lastH, w.numSlots * (uint64_t)w.maxCol);
 	w.maxRaw = maxCands * 4 < 1024 ? 1024 : maxCands * 4;
 	if(sc.local) rc |= xalloc(e, w.rawKeys, w.numSlots * (uint64_t)w.maxRaw);
-	w.o.maxCands = maxCands; w.o.maxAlns = maxAlns; w.o.maxOps = e->maxLen + 80;
+	w.o.maxCands = maxCands; w.o.maxAlns = maxAlns; w.o.maxOps = e->maxOps;
 	rc |= xalloc(e, w.o.probs, cap); rc |= xalloc(e, w.o.summ, cap); rc |= xalloc(e, w.o.cands, cap * (uint64_t)maxCands);
 	rc |= xalloc(e, w.o.alns, cap * (uint64_t)maxAlns); rc |= xalloc(e, w.o.ops, cap * (uint64_t)maxAlns * w.o.maxOps);
 	return rc;
@@ -454,10 +455,19 @@ int runBatch(bt2g_xengine *e, uint64_t nReads, const char *dNames, uint32_t name
 // maxPer = 0: one result row per read (bt2g_xengine_create); >= 1: the -k / -a entry arrays (bt2g_xengine_create_k)
 static int createEngine(bt2g_ctx *ctx, const bt2g_policy_params *pp, uint64_t maxUnits, uint32_t maxLen, uint32_t maxPer, bt2g_xengine **out) {
 	BT2G_CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+	// op rows (DP output, results, -k / -a entries): an alignment has one op per aligned row and one per read-gap column, and a read
+	// of l bases at most maxReadGaps(minsc(l), l) read gaps (every other position a match).  Under cheap read gaps, or a match bonus,
+	// that is several times l (--local --ma 3 --rdg 3,1); never narrower than the read + 80 of the default scorings
+	uint32_t maxOps = maxLen + 80;
+	{
+		XParams P; XTables T;
+		buildParams(pp, ctx->info.off_size, (int)maxLen, P, T);
+		for(int l = 1; l <= (int)maxLen; l++) maxOps = std::max<uint32_t>(maxOps, (uint32_t)(l + std::max(0, P.maxReadGaps(T.minsc[l], l))));
+	}
 	if(maxPer) {
 		// the dense arrays: rows of a result and an op string, pair records, entry counts
 		const uint64_t per = pp->paired ? 2 : 1, ents = maxUnits * (uint64_t)maxPer;
-		const uint64_t need = ents * per * (sizeof(bt2g_read_result) + maxLen + 80) + (pp->paired ? ents * sizeof(bt2g_pair_result) : 0) + maxUnits * 4;
+		const uint64_t need = ents * per * (sizeof(bt2g_read_result) + maxOps) + (pp->paired ? ents * sizeof(bt2g_pair_result) : 0) + maxUnits * 4;
 		size_t freeB = 0, totalB = 0;
 		BT2G_CUDA_TRY(ctx, cudaMemGetInfo(&freeB, &totalB));
 		if(need > freeB) {
@@ -472,7 +482,7 @@ static int createEngine(bt2g_ctx *ctx, const bt2g_policy_params *pp, uint64_t ma
 	if(!e) return -4;
 	e->ctx = ctx; e->pp = *pp; e->maxLen = (int)maxLen; e->maxUnits = maxUnits;
 	e->maxReads = pp->paired ? 2 * maxUnits : maxUnits; e->maxBases = e->maxReads * (uint64_t)maxLen;
-	e->maxOps = maxLen + 80;
+	e->maxOps = maxOps;
 	cudaDeviceGetAttribute(&e->sms, cudaDevAttrMultiProcessorCount, ctx->device);
 	if(const char *o = getenv("BT2G_XE_OCC")) e->stepOcc = atoi(o);          // experiment knob, read once
 	if(getenv("BT2G_XE_DEBUG")) e->debug = 1;
@@ -701,6 +711,8 @@ int bt2g_xengine_run_dev(bt2g_xengine *e, const uint8_t *dSeq, const uint8_t *dQ
 		bt2g_policy_params pp = e->pp; pp.host_threads = 8;
 		const int rc2 = bt2g_policy_align(&be, &pp, &sub, nptr.data(), res.data(), ops.data(), e->maxOps, paired ? prs.data() : nullptr, nullptr);
 		if(rc2 < 0) { ctx->err = "xengine: fallback engine failed"; return rc2; }
+		// (op rows hold the longest op string the scoring allows: a longer one would be a cut CIGAR / MD:Z, not a record)
+		for(const bt2g_read_result &r : res) if(r.nops > (int32_t)e->maxOps) { ctx->err = "xengine: fallback op string longer than the engine's op rows"; return -1; }
 		for(size_t j = 0; j < ids.size(); j++) {
 			const uint64_t r0 = ids[j] * per;
 			BT2G_CUDA_TRY(ctx, cudaMemcpy(e->d.res + r0, res.data() + j * per, per * sizeof(bt2g_read_result), cudaMemcpyHostToDevice));

@@ -1259,7 +1259,7 @@ class XEngine:
                        "bt2g_xengine_create_k")
         self._h = h
         self.paired = bool(params.paired)
-        self.max_ops = self.max_len + 80
+        self.max_ops = self.results_dev()[2]            # the engine's op rows: the longest op string the scoring allows
 
     def align(self, reads: ReadBatch, names=None, out: "HostBuffers" = None):
         """host buffers in -> (results, ops [n, max_ops], pairs or None, stats dict); with `out` the result arrays live in reused

@@ -155,6 +155,72 @@ class Reference(_Base):
         if not self.h:
             raise RuntimeError(f"reference: cannot open index {base}")
 
+    def set_scoring(self, sc):
+        """The handle's end-to-end (sc.local False) or local Scoring becomes the one the program builds from a
+        bowtie2_b200.policy.Scoring (--ma, --mp with quality-aware mismatches, --np, --rdg, --rfg, the gap barrier, --n-ceil,
+        --score-min); ref_dp / ref_ungapped / ref_one_mm use it from then on.  policy.Scoring.default(local) restores the default.
+
+        The reference library is built only where the reference's sources are, and that build is reused elsewhere, so this
+        goes through no new glue symbol: it writes the handle's own Scoring object (its plain data members and the three
+        penalty tables its constructor fills, _RefScoring) in place.  The layout is checked against the object's own
+        invariants before the write and against the reference's Scoring::maxReadGaps / maxRefGaps / perfectScore / nCeil
+        (ref_score_params) after it."""
+        from bowtie2_b200 import policy
+        local = bool(sc.local)
+        # RefHandle (oracle/ref_glue.cpp): unique_ptr<Ebwt> fw, bw; unique_ptr<BitPairReference> ref; unique_ptr<Scoring> sc_e2e, sc_loc
+        ptr = C.cast(C.c_void_p(self.h + 8 * (4 if local else 3)), C.POINTER(C.c_void_p)).contents.value
+        s = _RefScoring.from_address(ptr)
+        _RefScoring.check(s)
+        smin, nce = sc.score_min(), sc.n_ceil_func()
+        s.match_const, s.mmp_max, s.mmp_min, s.npen = sc.match_bonus, sc.mmp_max, sc.mmp_min, sc.n_pen
+        s.rd_gap_const, s.rf_gap_const, s.rd_gap_linear, s.rf_gap_linear, s.gapbar = (sc.rdgap_const, sc.rfgap_const, sc.rdgap_linear,
+                                                                                   sc.rfgap_linear, sc.gapbar)
+        s.monotone = sc.match_bonus == 0
+        big = np.finfo(np.float64).max
+        s.score_min = _RefSimpleFunc(smin.type, -big, big, float(smin.C), float(smin.L))
+        s.n_ceil = _RefSimpleFunc(policy.SIMPLE_FUNC_LINEAR, 0.0, big, float(nce.C), float(nce.L))
+        for q in range(256):                                   # Scoring::initPens
+            s.mmpens[q] = policy.mm_penalty(q, sc.mmp_max, sc.mmp_min)
+            s.npens[q] = sc.n_pen
+            s.match_bonuses[q] = float(sc.match_bonus)
+        _RefScoring.check(s)
+        out4 = np.zeros(4, np.int64)
+        f = self.lib.ref_score_params
+        f.argtypes = [vp, ci, C.c_int64, u64, vp]
+        f.restype = None
+        for rdlen in (20, 100, 250):
+            minsc = sc.min_score(rdlen)
+            f(self.h, int(local), minsc, rdlen, out4.ctypes.data_as(vp))
+            want = [sc.max_read_gaps(minsc, rdlen), sc.max_ref_gaps(minsc, rdlen), sc.perfect_score(rdlen), sc.n_ceil_raw(rdlen)]
+            if [int(x) for x in out4] != want:
+                raise RuntimeError(f"reference Scoring after set_scoring: {list(out4)} != {want} at {rdlen} bp")
+
+
+class _RefSimpleFunc(C.Structure):
+    _fields_ = [("type", ci), ("lo", C.c_double), ("hi", C.c_double), ("const", C.c_double), ("linear", C.c_double)]
+
+
+class _RefScoring(C.Structure):
+    """the data members of the reference's Scoring (scoring.h) up to its penalty tables, in declaration order (no virtual functions:
+    the first member is at offset 0)"""
+    _fields_ = [("match_type", ci), ("match_const", ci), ("mmcost_type", ci), ("mmp_max", ci), ("mmp_min", ci),
+                ("score_min", _RefSimpleFunc), ("n_ceil", _RefSimpleFunc), ("npen_type", ci), ("npen", ci), ("ncatpair", C.c_bool),
+                ("rd_gap_const", ci), ("rf_gap_const", ci), ("rd_gap_linear", ci), ("rf_gap_linear", ci), ("gapbar", ci),
+                ("monotone", C.c_bool), ("match_bonuses", C.c_float * 256), ("mmpens", ci * 256), ("npens", ci * 256)]
+    QUAL, CONSTANT = 2, 3          # COST_MODEL_QUAL, COST_MODEL_CONSTANT
+
+    @staticmethod
+    def check(s):
+        """the invariants the constructor leaves (quality-aware mismatches, constant N penalty and match bonus, tables filled from
+        the scalars): a member at another offset than assumed breaks them"""
+        from bowtie2_b200 import policy
+        ok = (s.match_type == _RefScoring.CONSTANT and s.mmcost_type == _RefScoring.QUAL and s.npen_type == _RefScoring.CONSTANT
+              and s.n_ceil.type == policy.SIMPLE_FUNC_LINEAR and 0 <= s.gapbar < 1 << 16 and s.monotone == (s.match_const == 0)
+              and all(s.mmpens[q] == policy.mm_penalty(q, s.mmp_max, s.mmp_min) for q in range(256))
+              and all(s.npens[q] == s.npen and s.match_bonuses[q] == s.match_const for q in range(256)))
+        if not ok:
+            raise RuntimeError("the reference's Scoring object does not have the layout oracle_lib._RefScoring assumes")
+
 
 # ---- DP through the unmodified SwAligner (oracle/ref_glue_dp.cpp) ------------------------------
 def ref_dp(R, local, codes, quals, fw, tidx, tlen, rect, minsc, rndseed=1234, max_cands=1024, max_alns=32, max_edits=4096):
@@ -193,6 +259,27 @@ class _OScoring(C.Structure):
 
 
 SCORING_OVERRIDE = None      # a bowtie2_b200.policy.Scoring: non-default penalties for the oracle calls that follow
+
+
+def scoring_grid():
+    """id -> policy.Scoring: the non-default scorings the DP, ungapped and 1-mismatch kernels are pinned to the reference under.
+    Flat and steep mismatch costs (the query profile, quality scaling); N penalties 0 (increments of 0: the edge of the
+    "every increment <= 0" arguments of the end-to-end fill) and 3; cheap, asymmetric and const < linear gaps (long gap walks, many
+    gap candidates, op strings longer than the read + 64); gap barriers 1 and 10; N ceilings of 0 and half the read; minimum
+    scores on both sides of the H-byte limit at 100 bp (1 - minsc <= 127); local with match bonuses 1 and 3 and cheap gaps."""
+    from bowtie2_b200 import policy
+    F, LIN, LOG = policy.SimpleFunc, policy.SIMPLE_FUNC_LINEAR, policy.SIMPLE_FUNC_LOG
+    e2e = {"mp6,6": dict(mmp_max=6, mmp_min=6), "mp2,2": dict(mmp_max=2, mmp_min=2), "mp8,3": dict(mmp_max=8, mmp_min=3),
+           "np0": dict(n_pen=0), "np3": dict(n_pen=3), "rdg1,1": dict(rdgap_const=1, rdgap_linear=1), "rfg1,1": dict(rfgap_const=1, rfgap_linear=1),
+           "rdg5,1-rfg8,4": dict(rdgap_const=5, rdgap_linear=1, rfgap_const=8, rfgap_linear=4), "rdg3,4": dict(rdgap_const=3, rdgap_linear=4),
+           "gapbar1": dict(gapbar=1), "gapbar10": dict(gapbar=10), "nceil-L0,0": dict(n_ceil_over=F(LIN, 0.0, 0.0)),
+           "nceil-L0,0.5": dict(n_ceil_over=F(LIN, 0.0, 0.5)), "minsc-126": dict(score_min_func=F(LIN, -126.0, 0.0)),
+           "minsc-127": dict(score_min_func=F(LIN, -127.0, 0.0))}
+    loc = {"local-ma1": dict(match_bonus=1, rdgap_const=2, rdgap_linear=1, rfgap_const=2, rfgap_linear=1, score_min_func=F(LOG, 10.0, 5.4)),
+           "local-ma3": dict(match_bonus=3, rdgap_const=3, rdgap_linear=1, rfgap_const=3, rfgap_linear=1, score_min_func=F(LOG, 20.0, 8.0))}
+    out = {k: policy.Scoring(**v) for k, v in e2e.items()}
+    out.update({k: policy.Scoring(local=True, **v) for k, v in loc.items()})
+    return out
 
 
 def oracle_scoring(O, local):

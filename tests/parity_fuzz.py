@@ -5,11 +5,13 @@ the engines take (--nofw/--norc, -L, -D, -R, -i, --ff/--rf, -I/-X, --dovetail, -
 --no-discordant, --mp, --np, --rdg, --rfg, --ma, --score-min, --n-ceil, --seed, -M; .bt2 and .bt2l indexes).  Every SAM record must be identical.
 
 Test infrastructure (uses oracle/): `python tests/parity_fuzz.py SEED CASES` prints one line per case and a JSON summary;
-tests/test_parity_fuzz.py runs a few fixed seeds."""
+tests/test_parity_fuzz.py runs a few fixed seeds.  With --device (a GPU) the same cases run on the device engine itself
+(bt2g_xengine_align / _align_k over the CUDA kernels); tests/test_xengine_fuzz_gpu.py runs a fixed list of them."""
 import json
 import os
 import subprocess
 import sys
+import tempfile
 import time
 
 import numpy as np
@@ -111,6 +113,7 @@ def draw_case(seed, k):
     c["straddle"] = bool(rng.random() < 0.3)
     c["read_seed"] = int(rng.integers(1, 1 << 30))
     c["kw"], c["flags"] = kw, flags
+    c["dense_sa"], c["seed_table"] = k % 3 == 1, k % 4 == 2        # device engine: the dense SA, a 12-mer seed table (longer than -L 10)
     return c
 
 
@@ -146,8 +149,44 @@ def _format_options(c, local):
     return {"sc": c["kw"]["sc"]} if "sc" in c["kw"] else {}
 
 
-def run_case(c, work, n_unpaired=300, n_pairs=200):
-    """-> (records, differing, first difference or None, engine stats, description)"""
+def _device_lines(c, base, batch, names, ref_names, fmt):
+    """the case on the device engine (bt2g_xengine_*: the state machine in waves over the CUDA kernels, at the engine's own op-row
+    width): align for -M, align_k + align.expand_entries for -k / -a.  -> (SAM records, (units, fallback units))"""
+    from bowtie2_b200 import Bt2Gpu
+    from bowtie2_b200.align import expand_entries, k_caps
+    from bowtie2_b200.lib import XEngine, load_library, policy_params, sam_format
+    lib = load_library()
+    paired, kw = c["paired"], c["kw"]
+    g = Bt2Gpu(0)
+    try:
+        g.load_index_files(base)
+        if c.get("dense_sa"):
+            g.build_dense_sa(0)
+        if c.get("seed_table"):
+            g.build_seed_table(12)
+        prm = policy_params(c["preset"], local=c["local"], paired=paired, seed=c.get("run_seed", 0), **kw)
+        units, max_len = batch.n // (2 if paired else 1), max(1, int(batch.lengths().max()))
+        cap = k_caps(kw, paired)
+        eng = XEngine(g, prm, units, max_len, max_per_unit=cap)
+        try:
+            if cap is None:
+                res, ops, pairs, st = eng.align(batch, names)
+                lines = sam_format(lib, batch, res, ops, ref_names, read_names=names, pairs=pairs, **fmt)
+            else:
+                res, ops, pairs, cnt, truncated, st = eng.align_k(batch, names)
+                assert not truncated
+                out = expand_entries(batch, names, res, ops, cnt, pairs)
+                lines = sam_format(lib, out[0], out[2], out[3], ref_names, read_names=out[1], pairs=out[4] if paired else None, **fmt)
+        finally:
+            eng.close()
+    finally:
+        g.close()
+    return lines.rstrip("\n").split("\n"), (units, st["fallback_units"])
+
+
+def run_case(c, work, n_unpaired=300, n_pairs=200, device=False):
+    """-> (records, differing, first difference or None, engine stats, description).  device: the device engine on the GPU
+    (_device_lines) instead of the state machine's host build over the C oracle's table"""
     import conftest
     from bowtie2_b200 import synth
     from bowtie2_b200.lib import ReadBatch, load_library, policy_align, policy_params, sam_format
@@ -185,7 +224,9 @@ def run_case(c, work, n_unpaired=300, n_pairs=200):
     from oracle_lib import Oracle, oracle_policy_table
     fmt = dict(local=local, no_discordant=(c["kw"].get("discord") is False), **_format_options(c, local))
     batch = ReadBatch.from_list(reads, quals)
-    if c["kw"].get("k") is not None or c["kw"].get("all_hits"):
+    if device:
+        lines, st = _device_lines(c, base, batch, names, ref_names, fmt)
+    elif c["kw"].get("k") is not None or c["kw"].get("all_hits"):
         # every reported alignment: align.py's own expansion of bt2g_policy_align_k / bt2g_policy_align_pairs_k over the C oracle's table
         from bowtie2_b200.align import _exact_batch
 
@@ -262,19 +303,24 @@ def run_case(c, work, n_unpaired=300, n_pairs=200):
 
 
 def main():
-    seed, cases = int(sys.argv[1]) if len(sys.argv) > 1 else 1, int(sys.argv[2]) if len(sys.argv) > 2 else 20
-    work = sys.argv[3] if len(sys.argv) > 3 else "/tmp/bt2g_parity_fuzz"
+    args = [a for a in sys.argv[1:] if a != "--device"]
+    device = "--device" in sys.argv[1:]
+    seed, cases = int(args[0]) if len(args) > 0 else 1, int(args[1]) if len(args) > 1 else 20
+    work = args[2] if len(args) > 2 else os.path.join(tempfile.gettempdir(), "bt2g_parity_fuzz")
     tot = bad = units = fallbacks = 0
     t0 = time.time()
     for k in range(cases):
         c = draw_case(seed, k)
-        n, nb, first, st, desc = run_case(c, work)
+        n, nb, first, st, desc = run_case(c, work, device=device)
         tot += n; bad += nb; units += st[0]; fallbacks += st[1]
-        print(f"case {k}: {desc}: {n} records, {nb} differing; {st[0]} units, {st[1]} finished by the coroutine engine", flush=True)
+        extra = "".join([" dense-SA" if c["dense_sa"] else "", " seed-table-12" if c["seed_table"] else ""]) if device else ""
+        print(f"case {k}: {desc}{extra}: {n} records, {nb} differing; {st[0]} units, {st[1]} finished by the coroutine engine", flush=True)
         if first:
             print("  GOT ", first[0][:300]); print("  WANT", first[1][:300])
     print(json.dumps({"seed": seed, "cases": cases, "records": tot, "differing": bad, "units": units, "host_fallbacks": fallbacks,
-                      "seconds": round(time.time() - t0, 1), "engine": "bt2g_xengine_align_host (csrc/xengine.cuh on the CPU, oracle-backed table)",
+                      "seconds": round(time.time() - t0, 1),
+                      "engine": ("bt2g_xengine_align / _align_k (the device engine on the CUDA kernels)" if device else
+                                 "bt2g_xengine_align_host (csrc/xengine.cuh on the CPU, oracle-backed table)"),
                       "reference": "oracle/_ref/bowtie2-align-s --seed 0 --reorder -p 1"}))
     return 1 if bad else 0
 

@@ -6,7 +6,8 @@ import pytest
 
 from bowtie2_b200 import policy, synth
 from bowtie2_b200.lib import DP_PROBLEM, ReadBatch, ops_to_edits
-from oracle_lib import Reference, have_reference, ref_dp
+import oracle_lib
+from oracle_lib import Oracle, Reference, have_reference, oracle_dp, ref_dp, scoring_grid
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(600)]
 
@@ -34,16 +35,27 @@ def _problems(genome, reads, truth, sc, jitter_rng, minsc_bump=0):
     return np.array(probs, dtype=DP_PROBLEM), meta
 
 
-def _check(gpu, R, genome, reads, quals, probs, meta, local=False, max_cands=None):
+def _check(gpu, R, genome, reads, quals, probs, meta, local=False, max_cands=None, sc=None, wants=None):
+    """bt2g_dp_extend against ref_dp problem by problem.  sc: a policy.Scoring the caller installed on both sides
+    (gpu.set_scoring_policy, R.set_scoring), which also sizes the op rows; wants: a dict that keeps the reference's answers
+    across calls on the same problems"""
     batch = ReadBatch.from_list(reads, quals)
-    summ, cands, alns, ops = gpu.dp_extend(batch, probs, max_cands=max_cands or (8192 if local else 256), max_alns=24 if local else 8,
-                                           max_ops=int(batch.lengths().max()) + 80)
+    max_ops = int(batch.lengths().max()) + 80
+    if sc is not None:
+        local = sc.local
+        max_ops = max([max_ops] + [len(reads[int(p["read_idx"])]) + sc.max_read_gaps(int(p["minsc"]), len(reads[int(p["read_idx"])])) for p in probs])
+    summ, cands, alns, ops = gpu.dp_extend(batch, probs, max_cands=max_cands or (8192 if local else 256),
+                                           max_alns=32 if sc is not None else (24 if local else 8), max_ops=max_ops)
     nfound = naln = ngap = 0
     for k, pr in enumerate(probs):
         tlen, rect, minsc = meta[k]
         i = int(pr["read_idx"])
-        want = ref_dp(R, local, reads[i], quals[i], int(pr["fw"]), int(pr["tidx"]), tlen, rect, minsc, max_cands=max(16384, max_cands or 0),
-                      max_alns=64, max_edits=16384)
+        want = None if wants is None else wants.get(k)
+        if want is None:
+            want = ref_dp(R, local, reads[i], quals[i], int(pr["fw"]), int(pr["tidx"]), tlen, rect, minsc, max_cands=max(16384, max_cands or 0),
+                          max_alns=64, max_edits=16384)
+            if wants is not None:
+                wants[k] = want
         s = summ[k]
         assert s["flags"] == 0, (k, s)
         assert bool(s["found"]) == bool(want["found"]), (k, s, want["found"], want["best"])
@@ -92,18 +104,22 @@ def test_dp_e2e_matches_reference(gpu, synth_index, synth_genome, rdlen, sub, in
 
 @pytest.mark.skipif(not have_reference(), reason="oracle/_ref not built")
 @pytest.mark.parametrize("mode", ["0", "1", "2"])
-def test_dp_e2e_kernel_generations(gpu, synth_index, synth_genome, mode, monkeypatch):
+def test_dp_e2e_kernel_generations(gpu, synth_index, synth_genome, mode):
     """The older end-to-end DP kernels (move codes 32-bit, move codes s16x2, fused H bytes) stay correct: they are the
-    fallbacks when a batch does not fit the split H-byte kernels (BT2G_DP_PACKED caps the mode)."""
-    import os
-    monkeypatch.setenv("BT2G_DP_PACKED", mode)
+    fallbacks when a batch does not fit the split H-byte kernels.  The context's mode cap (bt2g_set_dp_mode) selects them: a
+    100 bp read's default minimum score fits a byte, so each cap is the mode that runs."""
     gpu.load_index_files(synth_index)
     gpu.set_scoring(local=False)
     R = Reference(synth_index)
     sc = policy.Scoring.default(False)
     reads, quals, truth = synth.make_reads(synth_genome, 120, 100, seed=900 + int(mode), sub_rate=0.02, indel_rate=0.004)
     probs, meta = _problems(synth_genome, reads, truth, sc, np.random.default_rng(5))
-    nfound, naln, ngap = _check(gpu, R, synth_genome, reads, quals, probs, meta)
+    assert _kernel_mode(sc, int(probs["minsc"].min()), 100, int(mode)) == int(mode)
+    gpu.set_dp_mode(int(mode))
+    try:
+        nfound, naln, ngap = _check(gpu, R, synth_genome, reads, quals, probs, meta)
+    finally:
+        gpu.set_dp_mode(3)
     assert nfound > 80 and ngap > 3
 
 
@@ -157,3 +173,145 @@ def test_dp_local_matches_reference(gpu, synth_index, synth_genome, rdlen, sub, 
     nfound, naln, ngap = _check(gpu, R, synth_genome, reads, quals, probs, meta, local=True)
     assert nfound > 100 and naln > 100
     gpu.set_scoring(local=False)
+
+
+def _kernel_mode(sc, min_minsc, max_len, cap):
+    """dp_kernel_mode (dp_device.cuh): the end-to-end generation bt2g_dp_extend runs under the mode cap; "local" for local scoring"""
+    if sc.local:
+        return "local"
+    if cap == 0 or min_minsc < -8000 or sc.match_bonus * max_len > 8000:
+        return 0
+    rng = sc.match_bonus * max_len - (min_minsc - sc.match_bonus - 1)
+    return (3 if cap >= 3 else 2) if cap >= 2 and rng <= 127 else 1
+
+
+def _rows_per_lane(max_len, mode):
+    """dp_rows_per_lane (dp_device.cuh); the local kernels use the move-code rows"""
+    if mode in (2, 3):
+        return next(r for r in (4, 5, 6, 8, 10, 12, 16) if 32 * r >= max_len)
+    return 4 if max_len <= 128 else (8 if max_len <= 256 else 16)
+
+
+GRID_LENGTHS = [100, 150, 180, 250]        # 32 R >= length: R = 4, 5, 6, 8 on the H-byte kernels, 4 and 8 on the move-code kernels
+GRID_RAN = set()                           # (mode, rows per lane) of the grid's calls with found alignments
+
+
+@pytest.fixture(scope="module")
+def grid_mate_index(tmp_path_factory):
+    """the mate-window genome of test_dp_mate_gpu (tandem family, N gap, a short contig) and its index"""
+    import test_dp_mate_gpu
+    from conftest import _build_index
+    genome = test_dp_mate_gpu.make_mate_genome()
+    d = tmp_path_factory.mktemp("grid_mate")
+    synth.write_fasta(str(d / "g.fa"), genome)
+    _build_index("bowtie2-build-s", str(d / "g.fa"), str(d / "g"))
+    return genome, str(d / "g")
+
+
+def _grid_reads(genome, sc, L, seed, n_rich):
+    reads, quals, truth = synth.make_reads(genome, 40, L, seed=seed, sub_rate=0.02, indel_rate=0.006, random_frac=0.05)
+    rng = np.random.default_rng(seed)
+    for r in reads[:6]:
+        r[rng.integers(0, L)] = 4
+    if n_rich:
+        for r in reads[::2]:
+            r[rng.integers(0, L, int(rng.integers(1, 6)))] = 4
+    if sc.local:
+        for r in reads[::3]:
+            k = int(rng.integers(3, 15))
+            r[:k] = rng.integers(0, 4, k)
+    return reads, quals, truth, rng
+
+
+def _byte_bump(sc, L):
+    """end-to-end minimum scores below -127 are raised to -100 at the longest grid length, so that its rows-per-lane instantiation
+    of the H-byte kernels runs too (the move-code kernels run at every length)"""
+    return 0 if sc.local or sc.min_score(L) >= -127 or L < 250 else -100 - sc.min_score(L)
+
+
+def _caps_checked(gpu, R, genome, reads, quals, probs, meta, sc, L):
+    """the problems at every mode cap (local: its one generation), each against the reference; -> found problems per cap"""
+    found, wants = [], {}
+    for cap in ((3,) if sc.local else (0, 1, 2, 3)):
+        gpu.set_dp_mode(cap)
+        nfound, naln, _ = _check(gpu, R, genome, reads, quals, probs, meta, sc=sc, max_cands=16384 if sc.local else 2048, wants=wants)
+        mode = _kernel_mode(sc, int(probs["minsc"].min()), max(len(reads[int(i)]) for i in probs["read_idx"]), cap)
+        if nfound:
+            GRID_RAN.add((mode, _rows_per_lane(max(len(reads[int(i)]) for i in probs["read_idx"]), 0 if mode == "local" else mode)))
+        found.append((cap, mode, nfound, naln))
+    return found
+
+
+def _fates(gpu, O, reads, quals, probs, meta, sc, cap):
+    """candidate fates (SUCCEEDED / FAILED exactly where the reference starts a backtrace, in order) against oracle_dp's attempt log"""
+    gpu.set_dp_mode(cap)
+    summ, cands, _, _ = gpu.dp_extend(ReadBatch.from_list(reads, quals), probs, max_cands=32768 if sc.local else 2048, max_alns=32,
+                                      max_ops=max(len(r) for r in reads) + sc.max_read_gaps(int(probs["minsc"].min()), max(len(r) for r in reads)))
+    n_att = 0
+    for k, p in enumerate(probs):
+        i = int(p["read_idx"])
+        assert summ[k]["flags"] == 0, (k, summ[k])
+        d = oracle_dp(O, sc.local, reads[i], quals[i], bool(p["fw"]), int(p["tidx"]), meta[k][1], int(p["minsc"]), int(p["nceil"]),
+                      max_cands=65536, max_alns=64, max_edits=16384, attempts=True)
+        assert bool(summ[k]["found"]) == bool(d["found"]), k
+        if not d["found"]:
+            continue
+        got = [(ci, int(cands[k][ci]["fate"])) for ci in range(int(summ[k]["ncand"])) if int(cands[k][ci]["fate"]) in (2, 3)]
+        want = [(ci, 3 if ai >= 0 else 2) for (_, ai), ci in zip(d["attempts"], d["attempt_cands"])]
+        assert got == want, (k, got[:6], want[:6])
+        n_att += len(want)
+    return n_att
+
+
+@pytest.mark.skipif(not have_reference(), reason="oracle/_ref not built")
+@pytest.mark.parametrize("name", sorted(scoring_grid()))
+def test_dp_matches_reference_under_scoring(gpu, synth_index, synth_genome, grid_mate_index, name):
+    """Every DP kernel generation (mode caps 0-3) at R = 4, 5, 6 and 8 on seed-extension rectangles, and on mate windows at 150 bp,
+    against SwAligner under oracle_lib.scoring_grid()'s scorings; candidate fates against the C restatement's attempt log in
+    modes 1 and 3 (local: its kernel)"""
+    from test_dp_mate_gpu import _mate_problems
+    sc = scoring_grid()[name]
+    mate_genome, mate_base = grid_mate_index
+    default = policy.Scoring.default(sc.local)
+    try:
+        gpu.load_index_files(synth_index)
+        gpu.set_scoring_policy(sc)
+        R = Reference(synth_index)
+        R.set_scoring(sc)
+        seeds = 0
+        for L in GRID_LENGTHS:
+            reads, quals, truth, rng = _grid_reads(synth_genome, sc, L, 300 + L, name.startswith("nceil"))
+            probs, meta = _problems(synth_genome, reads, truth, sc, rng, minsc_bump=_byte_bump(sc, L))
+            per_cap = _caps_checked(gpu, R, synth_genome, reads, quals, probs, meta, sc, L)
+            assert all(nf > 10 and na > 10 for _, _, nf, na in per_cap), (L, per_cap)
+            seeds += per_cap[0][2]
+            if L == 100:
+                O = Oracle(synth_index)
+                oracle_lib.SCORING_OVERRIDE = sc
+                for cap in ((3,) if sc.local else (1, 3)):
+                    assert _fates(gpu, O, reads, quals, probs, meta, sc, cap) > 20
+                oracle_lib.SCORING_OVERRIDE = None
+        if name == "minsc-126":
+            assert per_cap[-1][1] == 3                              # 1 - minsc = 127: the H-byte kernels
+        if name == "minsc-127":
+            assert per_cap[-1][1] == 1                              # 128: the s16x2 move-code kernel
+        R.set_scoring(default)
+        gpu.load_index_files(mate_base)
+        gpu.set_scoring_policy(sc)
+        R = Reference(mate_base)
+        R.set_scoring(sc)
+        reads, quals, probs, meta = _mate_problems(mate_genome, 150, sc, np.random.default_rng(150))
+        per_cap = _caps_checked(gpu, R, mate_genome, reads, quals, probs, meta, sc, 150)
+        assert all(nf > 5 and na > 5 for _, _, nf, na in per_cap), per_cap
+        R.set_scoring(default)
+    finally:
+        oracle_lib.SCORING_OVERRIDE = None
+        gpu.set_dp_mode(3)
+        gpu.set_scoring(local=False)
+
+
+def test_dp_zz_every_grid_generation_ran():
+    """the end of the file: under the scoring grid every end-to-end generation ran with found alignments at every rows-per-lane
+    instantiation that reads of 100-250 bases reach, and the local kernel at both of its"""
+    want = {(0, 4), (0, 8), (1, 4), (1, 8)} | {(m, r) for m in (2, 3) for r in (4, 5, 6, 8)} | {("local", 4), ("local", 8)}
+    assert want <= GRID_RAN, sorted(want - GRID_RAN, key=str)

@@ -25,6 +25,10 @@ def _mutate(rng, seq, n):
 
 @pytest.fixture(scope="module")
 def mate_genome():
+    return make_mate_genome()
+
+
+def make_mate_genome():
     rng = np.random.default_rng(2026)
     c0 = rng.integers(0, 4, 30000).astype(np.uint8)
     unit = rng.integers(0, 4, UNIT).astype(np.uint8)

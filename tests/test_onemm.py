@@ -3,7 +3,11 @@ import numpy as np
 import pytest
 
 from bowtie2_b200 import synth
-from oracle_lib import Oracle, Reference, have_reference, oracle_one_mm, ref_one_mm
+import oracle_lib
+from oracle_lib import Oracle, Reference, have_reference, oracle_one_mm, ref_one_mm, scoring_grid
+
+# the scorings of oracle_lib.scoring_grid() that the 1-mismatch search reads: mismatch and N penalties, the match bonus
+GRID = ["mp6,6", "mp2,2", "mp8,3", "np0", "np3", "local-ma1", "local-ma3"]
 
 
 def _cases(genome, seed=33):
@@ -34,27 +38,57 @@ def _minsc(ln, local, k):
 @pytest.mark.skipif(not have_reference(), reason="oracle/_ref not built")
 @pytest.mark.parametrize("local", [False, True])
 def test_onemm_oracle_vs_reference(local, synth_index, synth_genome):
+    assert _oracle_vs_reference(Oracle(synth_index), Reference(synth_index), local, synth_genome) > 50
+
+
+@pytest.mark.skipif(not have_reference(), reason="oracle/_ref not built")
+@pytest.mark.parametrize("name", GRID)
+def test_onemm_oracle_vs_reference_under_scoring(name, synth_index, synth_genome):
+    sc = scoring_grid()[name]
     O, R = Oracle(synth_index), Reference(synth_index)
+    R.set_scoring(sc)
+    oracle_lib.SCORING_OVERRIDE = sc
+    try:
+        assert _oracle_vs_reference(O, R, sc.local, synth_genome) > 50
+    finally:
+        oracle_lib.SCORING_OVERRIDE = None
+
+
+def _oracle_vs_reference(O, R, local, genome):
     nhit = 0
-    for k, (r, q) in enumerate(_cases(synth_genome)):
+    for k, (r, q) in enumerate(_cases(genome)):
         minsc = _minsc(len(r), local, k)
         nofw, norc = (k % 11 == 5), (k % 13 == 7)
         a = oracle_one_mm(O, local, r, q, minsc, nofw, norc)
         b = ref_one_mm(R, local, r, q, minsc, nofw, norc)
         assert a == b, (k, len(r), a, b)
         nhit += len(a)
-    assert nhit > 50
+    return nhit
 
 
 @pytest.mark.gpu
 @pytest.mark.timeout(300)
-@pytest.mark.parametrize("which,local", [("small", False), ("small", True), ("large", False)])
-def test_onemm_gpu_vs_oracle(which, local, gpu, synth_index, synth_index_large, synth_genome):
-    from bowtie2_b200.lib import ReadBatch
+@pytest.mark.parametrize("which,local,scoring", [pytest.param("small", False, None, id="small-False"), pytest.param("small", True, None, id="small-True"),
+                                                 pytest.param("large", False, None, id="large-False")] +
+                         [pytest.param("small", name.startswith("local"), name, id="small-" + name) for name in ("mp8,3", "mp2,2", "np0", "local-ma3")])
+def test_onemm_gpu_vs_oracle(which, local, scoring, gpu, synth_index, synth_index_large, synth_genome):
+    """the kernel and the restatement under the default scorings and, as gpu.set_scoring_policy installs them, some of the grid's"""
     base = synth_index if which == "small" else synth_index_large
     gpu.load_index_files(base)
-    gpu.set_scoring(local=local)
-    O = Oracle(base)
+    if scoring is None:
+        gpu.set_scoring(local=local)
+    else:
+        oracle_lib.SCORING_OVERRIDE = scoring_grid()[scoring]
+        gpu.set_scoring_policy(oracle_lib.SCORING_OVERRIDE)
+    try:
+        _gpu_vs_oracle(gpu, Oracle(base), local, synth_genome)
+    finally:
+        oracle_lib.SCORING_OVERRIDE = None
+        gpu.set_scoring(local=False)
+
+
+def _gpu_vs_oracle(gpu, O, local, synth_genome):
+    from bowtie2_b200.lib import ReadBatch
     cases = _cases(synth_genome)
     batch = ReadBatch.from_list([c[0] for c in cases], quals=[c[1] for c in cases])
     minsc = np.array([_minsc(len(c[0]), local, k) for k, c in enumerate(cases)], dtype=np.int32)
@@ -72,5 +106,4 @@ def test_onemm_gpu_vs_oracle(which, local, gpu, synth_index, synth_index_large, 
         # the reference appends per (strand, index) pass in loop order; the kernel keeps one list per pass
         assert got == want, (k, len(r), got, want)
         nhit += len(got)
-    gpu.set_scoring(local=False)
     assert nhit > 50

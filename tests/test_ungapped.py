@@ -3,7 +3,11 @@ import numpy as np
 import pytest
 
 from bowtie2_b200 import synth
-from oracle_lib import Oracle, Reference, have_reference, oracle_ungapped, ref_ungapped
+import oracle_lib
+from oracle_lib import Oracle, Reference, have_reference, oracle_ungapped, ref_ungapped, scoring_grid
+
+# the scorings of oracle_lib.scoring_grid() that the ungapped aligner reads: mismatch and N penalties, the N ceiling, the match bonus
+GRID = ["mp6,6", "mp2,2", "mp8,3", "np0", "np3", "nceil-L0,0", "nceil-L0,0.5", "local-ma1", "local-ma3"]
 
 
 def _cases(genome, n=400, seed=77):
@@ -54,12 +58,9 @@ def _ref_view(rc, d, ln, fw):
     return (d["score"], d["refoff"], rowi, rowf, d["ns"], d["refns"], rows)
 
 
-@pytest.mark.skipif(not have_reference(), reason="oracle/_ref not built")
-@pytest.mark.parametrize("local", [False, True])
-def test_ungapped_oracle_vs_reference(local, synth_index, synth_genome):
-    O, R = Oracle(synth_index), Reference(synth_index)
+def _oracle_vs_reference(O, R, local, genome):
     seen = set()
-    for k, (r, q, fw, t, off, tlen, ohang) in enumerate(_cases(synth_genome)):
+    for k, (r, q, fw, t, off, tlen, ohang) in enumerate(_cases(genome)):
         minsc = _minsc(len(r), local, k)
         rc, d = ref_ungapped(R, local, r, q, fw, t, off, tlen, ohang, minsc)
         oc, od = oracle_ungapped(O, local, r, q, fw, t, off, tlen, ohang, minsc)
@@ -69,18 +70,53 @@ def test_ungapped_oracle_vs_reference(local, synth_index, synth_genome):
             want = _ref_view(rc, d, len(r), fw)
             got = (od["score"], off + od["rowi"], od["rowi"], od["rowf"], od["ns"], od["refns"], sorted(np.nonzero(od["mask"])[0].tolist()))
             assert got == want, (k, got, want)
+    return seen
+
+
+@pytest.mark.skipif(not have_reference(), reason="oracle/_ref not built")
+@pytest.mark.parametrize("local", [False, True])
+def test_ungapped_oracle_vs_reference(local, synth_index, synth_genome):
+    seen = _oracle_vs_reference(Oracle(synth_index), Reference(synth_index), local, synth_genome)
     assert 0 in seen and 1 in seen and (not local or -1 in seen or True)
+
+
+@pytest.mark.skipif(not have_reference(), reason="oracle/_ref not built")
+@pytest.mark.parametrize("name", GRID)
+def test_ungapped_oracle_vs_reference_under_scoring(name, synth_index, synth_genome):
+    sc = scoring_grid()[name]
+    O, R = Oracle(synth_index), Reference(synth_index)
+    R.set_scoring(sc)
+    oracle_lib.SCORING_OVERRIDE = sc
+    try:
+        seen = _oracle_vs_reference(O, R, sc.local, synth_genome)
+    finally:
+        oracle_lib.SCORING_OVERRIDE = None
+    assert 0 in seen and 1 in seen
 
 
 @pytest.mark.gpu
 @pytest.mark.timeout(300)
-@pytest.mark.parametrize("which,local", [("small", False), ("small", True), ("large", False)])
-def test_ungapped_gpu_vs_oracle(which, local, gpu, synth_index, synth_index_large, synth_genome):
-    from bowtie2_b200.lib import ReadBatch, UNGAPPED_PROBLEM
+@pytest.mark.parametrize("which,local,scoring", [pytest.param("small", False, None, id="small-False"), pytest.param("small", True, None, id="small-True"),
+                                                 pytest.param("large", False, None, id="large-False")] +
+                         [pytest.param("small", name.startswith("local"), name, id="small-" + name) for name in ("mp8,3", "mp2,2", "np0", "nceil-L0,0", "local-ma3")])
+def test_ungapped_gpu_vs_oracle(which, local, scoring, gpu, synth_index, synth_index_large, synth_genome):
+    """the kernel and the restatement under the default scorings and, as gpu.set_scoring_policy installs them, some of the grid's"""
     base = synth_index if which == "small" else synth_index_large
     gpu.load_index_files(base)
-    gpu.set_scoring(local=local)
-    O = Oracle(base)
+    if scoring is None:
+        gpu.set_scoring(local=local)
+    else:
+        oracle_lib.SCORING_OVERRIDE = scoring_grid()[scoring]
+        gpu.set_scoring_policy(oracle_lib.SCORING_OVERRIDE)
+    try:
+        _gpu_vs_oracle(gpu, Oracle(base), local, synth_genome)
+    finally:
+        oracle_lib.SCORING_OVERRIDE = None
+        gpu.set_scoring(local=False)
+
+
+def _gpu_vs_oracle(gpu, O, local, synth_genome):
+    from bowtie2_b200.lib import ReadBatch, UNGAPPED_PROBLEM
     cases = _cases(synth_genome)
     batch = ReadBatch.from_list([c[0] for c in cases], quals=[c[1] for c in cases])
     probs = np.zeros(len(cases), dtype=UNGAPPED_PROBLEM)
@@ -97,5 +133,4 @@ def test_ungapped_gpu_vs_oracle(which, local, gpu, synth_index, synth_index_larg
             assert (int(g["score"]), int(g["rowi"]), int(g["rowf"]), int(g["ns"]), int(g["refns"]), int(g["nedits"])) == \
                    (od["score"], od["rowi"], od["rowf"], od["ns"], od["refns"], od["nedits"]), k
             assert np.array_equal(mask[k, :len(r)], od["mask"]), k
-    gpu.set_scoring(local=False)
     assert nfound > 50

@@ -151,3 +151,38 @@ def test_text_stream_over_device_engines(request):
     bad = [i for i in range(len(golden)) if lines[i] != golden[i]]
     assert written == 2 * n and not bad, (written, len(bad), lines[bad[0]] if bad else None)
     g.close()
+
+
+@pytest.mark.parametrize("paired,flag", [(False, "nofw"), (False, "norc"), (True, "nofw"), (True, "norc")])
+def test_device_engine_skips_the_strands_of_nofw_norc(tmp_path, paired, flag):
+    """--nofw / --norc: the seed search of a wave skips the strand a unit's mate may not align to, as the reference's
+    instantiateSeeds does (the device's seed wave once searched both strands of every read: most records differed)"""
+    from bowtie2_b200 import synth
+    from oracle_lib import have_reference, ref_bin
+    if not have_reference():
+        pytest.skip("oracle/_ref not built")
+    g = _gpu()
+    genome = synth.make_genome(n_contigs=2, contig_len=40000, seed=5, repeat_frac=0.1, repeat_len=300, repeat_copies=8, n_gap=20)
+    fa, base = str(tmp_path / "g.fa"), str(tmp_path / "g")
+    synth.write_fasta(fa, genome)
+    subprocess.check_call([ref_bin("bowtie2-build-s"), "--seed", "0", "--quiet", fa, base])
+    n = 300
+    if paired:
+        reads, quals, _ = synth.make_pairs(genome, n, 100, seed=8, sub_rate=0.03, indel_rate=0.002, ins_mean=300, ins_sd=40)
+        f1, f2 = str(tmp_path / "r1.fq"), str(tmp_path / "r2.fq")
+        synth.write_fastq(f1, reads[0::2], quals[0::2]); synth.write_fastq(f2, reads[1::2], quals[1::2])
+        io = ["-1", f1, "-2", f2]
+    else:
+        reads, quals, _ = synth.make_reads(genome, n, 100, seed=8, sub_rate=0.03, indel_rate=0.002)
+        fq = str(tmp_path / "r.fq")
+        synth.write_fastq(fq, reads, quals)
+        io = ["-U", fq]
+    out = subprocess.check_output([ref_bin("bowtie2-align-s"), "--sensitive", "--" + flag, "--seed", "0", "-p", "1", "--reorder", "-x", base] + io,
+                                  stderr=subprocess.DEVNULL).decode()
+    want = [l for l in out.split("\n") if l and not l.startswith("@")]
+    g.load_index_files(base)
+    lines, stats = _run(g, reads, quals, None, "sensitive", paired, False, ["chr1", "chr2"], **{flag: True})
+    bad = [i for i in range(len(want)) if lines[i] != want[i]]
+    assert len(lines) == len(want) and not bad, (len(bad), lines[bad[0]] if bad else None, want[bad[0]] if bad else None, stats)
+    assert sum(int(l.split("\t")[1]) & 4 == 0 for l in want) > len(want) // 3
+    g.close()
