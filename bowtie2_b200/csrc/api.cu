@@ -243,7 +243,6 @@ int bt2g_create(int device, bt2g_ctx **out) {
 		delete ctx; return -2;
 	}
 	// experiment knob: L2 -> HBM fetch granularity hint for the random 64 B side gathers
-	if(const char *m = getenv("BT2G_DP_PACKED")) if(m[0] >= '0' && m[0] <= '3') ctx->dpModeCap = m[0] - '0';   // experiment knob, read once
 	if(const char *g = getenv("BT2G_L2_FETCH")) cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, (size_t)atoi(g));
 	*out = ctx;
 	return 0;
@@ -682,7 +681,7 @@ int bt2g_dp_extend(bt2g_ctx *ctx, const bt2g_reads *reads, const bt2g_dp_problem
 	// (columns are 16-bit in the kernels; the mate windows of -X 8000 are about 8200 wide, and the kernels take fewer warps per
 	// block as windows widen)
 	if(maxCol > 16384) { ctx->err = "DP window wider than 16384 columns"; return -1; }
-	DBuf dseq, dqual, doff, dprob, dcodes, dlast, dsumm, dcand, daln, dops, draw, dctr;
+	DBuf dseq, dqual, doff, dprob, dcodes, dsumm, dcand, daln, dops, draw, dctr;
 	int rc = uploadReads(ctx, reads, dseq, dqual, doff, true);
 	if(rc) return rc;
 	DpLaunch L;
@@ -692,21 +691,13 @@ int bt2g_dp_extend(bt2g_ctx *ctx, const bt2g_reads *reads, const bt2g_dp_problem
 		uint64_t want = (uint64_t)sms * 24;      // 24 resident warps per SM
 		L.numSlots = ((n < want ? n : want) + 3) / 4 * 4;
 	} L.maxCands = maxCands; L.maxAlns = maxAlns; L.maxOps = maxOps;
-	L.packed = ctx->scoring.local ? 0 : dp_kernel_mode(ctx->scoring, minMinsc, maxLen, ctx->dpModeCap);
-	L.codeStride = dp_code_stride(maxCol, maxLen, L.packed);
+	const DpPlan P = dp_plan(ctx->scoring, minMinsc, maxLen, maxCol, n, L.numSlots, maxCands * 4 < 1024 ? 1024 : maxCands * 4,
+	                         ctx->dpModeCap, 6ull << 30);
+	L.mode = P.mode; L.codeStride = P.codeStride; L.chunk = P.chunk; L.maxRaw = P.maxRaw;
 	BT2G_CUDA_TRY(ctx, dprob.alloc(n * sizeof(bt2g_dp_problem)));
-	if(L.packed == 3) {
-		L.chunk = dp_chunk_problems(L.codeStride, n);
-		BT2G_CUDA_TRY(ctx, dcodes.alloc(L.chunk * L.codeStride));
-		BT2G_CUDA_TRY(ctx, dctr.alloc(4 * sizeof(uint32_t)));
-		L.taskCtr = dctr.as<uint32_t>();
-	} else {
-		BT2G_CUDA_TRY(ctx, dcodes.alloc(L.numSlots * L.codeStride * (L.packed ? 2 : 1)));
-	}
-	BT2G_CUDA_TRY(ctx, dlast.alloc(L.numSlots * (uint64_t)maxCol * 4));
-	L.maxRaw = maxCands * 4 < 1024 ? 1024 : maxCands * 4;
-	BT2G_CUDA_TRY(ctx, draw.alloc(L.numSlots * (uint64_t)L.maxRaw * 8));
-	L.rawKeys = draw.as<uint64_t>();
+	BT2G_CUDA_TRY(ctx, dcodes.alloc(P.codeBytes));
+	if(P.taskCtr) { BT2G_CUDA_TRY(ctx, dctr.alloc(4 * sizeof(uint32_t))); L.taskCtr = dctr.as<uint32_t>(); }
+	if(P.rawKeys) { BT2G_CUDA_TRY(ctx, draw.alloc(P.rawKeys * sizeof(uint64_t))); L.rawKeys = draw.as<uint64_t>(); }
 	BT2G_CUDA_TRY(ctx, dsumm.alloc(n * sizeof(bt2g_dp_summary)));
 	BT2G_CUDA_TRY(ctx, dcand.alloc(n * (uint64_t)maxCands * sizeof(bt2g_dp_cand)));
 	BT2G_CUDA_TRY(ctx, daln.alloc(n * (uint64_t)maxAlns * sizeof(bt2g_dp_aln)));
@@ -715,7 +706,7 @@ int bt2g_dp_extend(bt2g_ctx *ctx, const bt2g_reads *reads, const bt2g_dp_problem
 	BT2G_CUDA_TRY(ctx, cudaMemsetAsync(dcand.p, 0, dcand.bytes, ctx->stream));
 	BT2G_CUDA_TRY(ctx, cudaMemsetAsync(daln.p, 0, daln.bytes, ctx->stream));
 	L.seq = dseq.as<uint8_t>(); L.qual = dqual.as<uint8_t>(); L.roff = doff.as<uint64_t>();
-	L.probs = dprob.as<bt2g_dp_problem>(); L.codes = dcodes.as<uint8_t>(); L.lastH = dlast.as<int32_t>();
+	L.probs = dprob.as<bt2g_dp_problem>(); L.codes = dcodes.as<uint8_t>();
 	L.summ = dsumm.as<bt2g_dp_summary>(); L.cands = dcand.as<bt2g_dp_cand>(); L.alns = daln.as<bt2g_dp_aln>(); L.ops = dops.as<uint8_t>();
 	int lrc;
 	if(ctx->scoring.local) {

@@ -45,7 +45,7 @@ struct PipeBufs {
 	uint32_t *nRows, *rowBase, *rowCnt;
 	uint64_t *tidx, *textoff, *tlen; uint8_t *rflags;   // resolve
 	bt2g_dp_problem *probs; uint32_t *nProb; int32_t *readProb; int32_t *readNProb;
-	uint8_t *codes; int32_t *lastH; uint64_t *rawKeys; uint32_t *dpTasks;   // dpTasks: task counters of the split DP kernels
+	uint8_t *codes; uint64_t *rawKeys; uint32_t *dpTasks;   // dpTasks: task counters of the split DP kernels
 	bt2g_dp_summary *summ; bt2g_dp_cand *cands; bt2g_dp_aln *alns; uint8_t *ops;
 	bt2g_read_result *res; uint8_t *resOps;
 	unsigned long long *counters;             // [4]: sweep sides, seed sides, resolve sides, dp cells
@@ -63,12 +63,12 @@ struct bt2g_pipeline {
 	uint64_t maxReads, maxBases;
 	PipeBufs b;
 	std::vector<void *> allocs;
-	uint64_t numSlots, codeStride, maxProbs;
-	int packed = 0;                           // DP kernel mode (dp_kernel_mode)
-	uint64_t dpChunk = 0, mateChunk = 0;      // mode 3: problems per fill/tail chunk
-	int maxCol, R, sms = 148;
+	uint64_t numSlots, maxProbs;
+	DpPlan dp, mateDp;                        // the DP workspace plans of the anchor and the mate pass (one workspace serves both)
+	int64_t minMinsc = 0;                     // the lowest minimum score of any read length (dp_plan)
+	int maxCol, sms = 148;
 	cudaEvent_t ev[9], pev[4];
-	bool pairsOn = false; bt2g_pe_policy pe{}; int mateMaxCol = 0; uint64_t mateCodeStride = 0;
+	bool pairsOn = false; bt2g_pe_policy pe{}; int mateMaxCol = 0;
 	bt2g_pair_result *hPairs = nullptr;
 	bool evOk = false;
 	// pinned staging for the host entry point
@@ -434,9 +434,9 @@ static int runStages(bt2g_pipeline *p, const uint8_t *seq, const uint8_t *qual, 
 	                               b.probs, b.nProb, (uint32_t)p->maxProbs, b.readProb, b.readNProb, b.res + resBase, b.probTlen, b.resTlen + resBase);
 	DpLaunch L;
 	L.seq = seq; L.qual = qual; L.roff = roff; L.probs = b.probs; L.n = p->maxProbs; L.nDev = b.nProb;
-	L.rawKeys = b.rawKeys; L.maxRaw = b.rawKeys ? PIPE_MAX_RAW : 0;
-	L.numSlots = p->numSlots; L.codes = b.codes; L.lastH = b.lastH; L.codeStride = p->codeStride; L.maxCol = p->maxCol;
-	L.maxCands = q.max_cands; L.maxAlns = q.max_alns; L.maxOps = q.max_ops; L.packed = p->packed; L.chunk = p->dpChunk; L.taskCtr = b.dpTasks;
+	L.rawKeys = b.rawKeys; L.maxRaw = p->dp.maxRaw;
+	L.numSlots = p->numSlots; L.codes = b.codes; L.codeStride = p->dp.codeStride; L.maxCol = p->maxCol;
+	L.maxCands = q.max_cands; L.maxAlns = q.max_alns; L.maxOps = q.max_ops; L.mode = p->dp.mode; L.chunk = p->dp.chunk; L.taskCtr = b.dpTasks;
 	L.summ = b.summ; L.cands = b.cands; L.alns = b.alns; L.ops = b.ops;
 	mark(6);
 	const int drc = p->sc.local ? launch_dp_local<OFF>(ix, p->sc, L, q.max_len, st) : launch_dp_e2e<OFF>(ix, p->sc, L, q.max_len, st);
@@ -469,9 +469,8 @@ static int runPairTail(bt2g_pipeline *p, const uint8_t *seq, const uint8_t *qual
 	cudaEventRecord(p->pev[1], st);
 	DpLaunch L;
 	L.seq = seq; L.qual = qual; L.roff = roff; L.probs = b.mProbs; L.n = p->maxReads; L.nDev = b.nMateProb;
-	L.rawKeys = nullptr; L.maxRaw = 0;
-	L.numSlots = p->numSlots; L.codes = b.codes; L.lastH = nullptr; L.codeStride = p->mateCodeStride; L.maxCol = p->mateMaxCol;
-	L.maxCands = q.max_cands; L.maxAlns = q.max_alns; L.maxOps = q.max_ops; L.packed = p->packed; L.chunk = p->mateChunk; L.taskCtr = b.dpTasks;
+	L.numSlots = p->numSlots; L.codes = b.codes; L.codeStride = p->mateDp.codeStride; L.maxCol = p->mateMaxCol;
+	L.maxCands = q.max_cands; L.maxAlns = q.max_alns; L.maxOps = q.max_ops; L.mode = p->mateDp.mode; L.chunk = p->mateDp.chunk; L.taskCtr = b.dpTasks;
 	L.summ = b.mSumm; L.cands = b.mCands; L.alns = b.mAlns; L.ops = b.mOps;
 	if(launch_dp_e2e<OFF>(ix, p->sc, L, q.max_len, st)) { ctx->err = "pipeline: mate DP launch rejected"; return -1; }
 	cudaEventRecord(p->pev[2], st);
@@ -518,25 +517,15 @@ int bt2g_pipeline_create(bt2g_ctx *ctx, const bt2g_pipeline_params *prm, uint64_
 	int sms = 148; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, ctx->device);
 	p->sms = sms;
 	p->numSlots = (uint64_t)sms * 24;
-	{
-		int64_t mn = 0;
-		for(int l = 1; l <= prm->max_len; l++) if(prm->minsc_by_len[l] < mn) mn = prm->minsc_by_len[l];
-		p->packed = p->sc.local ? 0 : dp_kernel_mode(p->sc, mn, prm->max_len, ctx->dpModeCap);
-	}
-	p->R = dp_rows_per_lane(prm->max_len, p->packed);
-	p->codeStride = dp_code_stride(p->maxCol, prm->max_len, p->packed);
-	if(p->packed == 3) {
-		p->dpChunk = dp_chunk_problems(p->codeStride, nprobMax);
-		rc |= pipeAlloc(p, b.codes, p->dpChunk * p->codeStride);
-	} else {
-		rc |= pipeAlloc(p, b.codes, p->numSlots * p->codeStride * (p->packed ? 2 : 1));
-	} rc |= pipeAlloc(p, b.lastH, p->numSlots * (uint64_t)p->maxCol);
-	// local mode gathers candidate cells during the fill (k_dp_local): a raw key list per warp slot
-	if(ctx->scoring.local) rc |= pipeAlloc(p, b.rawKeys, p->numSlots * (uint64_t)PIPE_MAX_RAW);
+	for(int l = 1; l <= prm->max_len; l++) if(prm->minsc_by_len[l] < p->minMinsc) p->minMinsc = prm->minsc_by_len[l];
+	p->dp = dp_plan(p->sc, p->minMinsc, prm->max_len, p->maxCol, nprobMax, p->numSlots, PIPE_MAX_RAW, ctx->dpModeCap, 6ull << 30);
+	rc |= pipeAlloc(p, b.codes, p->dp.codeBytes);
+	if(p->dp.rawKeys) rc |= pipeAlloc(p, b.rawKeys, p->dp.rawKeys);
 	rc |= pipeAlloc(p, b.summ, nprobMax); rc |= pipeAlloc(p, b.cands, nprobMax * prm->max_cands);
 	rc |= pipeAlloc(p, b.alns, nprobMax * prm->max_alns); rc |= pipeAlloc(p, b.ops, nprobMax * prm->max_alns * (uint64_t)prm->max_ops);
 	rc |= pipeAlloc(p, b.res, n); rc |= pipeAlloc(p, b.resOps, n * (uint64_t)prm->max_ops);
-	rc |= pipeAlloc(p, b.counters, 4); rc |= pipeAlloc(p, b.dpTasks, 4);
+	rc |= pipeAlloc(p, b.counters, 4);
+	if(p->dp.taskCtr) rc |= pipeAlloc(p, b.dpTasks, 4);
 	rc |= pipeAlloc(p, b.probTlen, nprobMax); rc |= pipeAlloc(p, b.resTlen, n);
 	if(rc) { bt2g_pipeline_destroy(p); return -2; }
 	cudaError_t e = cudaSuccess;
@@ -664,23 +653,18 @@ int bt2g_pipeline_enable_pairs(bt2g_pipeline *p, const bt2g_pe_policy *pol) {
 	const int maxgap = q.maxhalf > 32 ? q.maxhalf : 32;
 	p->mateMaxCol = (int)(maxfrag + q.max_len + 2 * maxgap + 8);
 	if(p->mateMaxCol > 8192) { ctx->err = "pipeline: -X too large for the mate-finding workspace"; return -1; }
-	p->mateCodeStride = dp_code_stride(p->mateMaxCol, q.max_len, p->packed);
+	// the mate pass runs the anchor pass's generation: its mode is the cap
+	const DpPlan M = dp_plan(p->sc, p->minMinsc, q.max_len, p->mateMaxCol, n, p->numSlots, 0, p->dp.mode, 6ull << 30);
 	int rc = 0;
 	uint8_t *codes2 = nullptr;
-	if(p->packed == 3) {
-		p->mateChunk = dp_chunk_problems(p->mateCodeStride, n);
-		const uint64_t need = p->mateChunk * p->mateCodeStride, have = p->dpChunk * p->codeStride;
-		rc |= pipeAlloc(p, codes2, need > have ? need : have);
-	} else {
-		rc |= pipeAlloc(p, codes2, p->numSlots * p->mateCodeStride * (p->packed ? 2 : 1));
-	}
+	rc |= pipeAlloc(p, codes2, M.codeBytes > p->dp.codeBytes ? M.codeBytes : p->dp.codeBytes);
 	rc |= pipeAlloc(p, b.mProbs, n); rc |= pipeAlloc(p, b.nMateProb, 1); rc |= pipeAlloc(p, b.mateOfRead, n);
 	rc |= pipeAlloc(p, b.mSumm, n); rc |= pipeAlloc(p, b.mCands, n * q.max_cands);
 	rc |= pipeAlloc(p, b.mAlns, n * q.max_alns); rc |= pipeAlloc(p, b.mOps, n * q.max_alns * (uint64_t)q.max_ops);
 	rc |= pipeAlloc(p, b.pairs, n / 2 + 1); rc |= pipeAlloc(p, b.mateCells, 1);
 	if(rc) return -2;
-	b.codes = codes2;        // the wider workspace serves both DP passes
-	if(p->packed != 3) p->codeStride = p->mateCodeStride;
+	b.codes = codes2;        // the larger workspace serves both DP passes
+	p->mateDp = M;
 	cudaError_t e = cudaMemset(b.mAlns, 0, n * q.max_alns * sizeof(bt2g_dp_aln));
 	if(e == cudaSuccess) e = cudaMemset(b.mCands, 0, n * q.max_cands * sizeof(bt2g_dp_cand));
 	if(e == cudaSuccess) e = cudaHostAlloc((void **)&p->hPairs, (n / 2 + 1) * sizeof(bt2g_pair_result), cudaHostAllocDefault);
@@ -788,12 +772,12 @@ int bt2g_pipeline_pair_stage_ms(bt2g_pipeline *p, float *out3) {
 int bt2g_pipeline_kernel_launches(bt2g_pipeline *p) {
 	if(!p) return -1;
 	int dp = 1;
-	if(p->packed == 3 && p->dpChunk) dp = 2 * (int)((p->maxProbs + p->dpChunk - 1) / p->dpChunk);
+	if(p->dp.chunk) dp = 2 * (int)((p->maxProbs + p->dp.chunk - 1) / p->dp.chunk);
 	int pe = 0;
 	if(p->pairsOn) {
 		// k_frame_mates, the mate DP kernel(s), k_pick_pairs
 		int mdp = 1;
-		if(p->packed == 3 && p->mateChunk) mdp = 2 * (int)((p->maxReads + p->mateChunk - 1) / p->mateChunk);
+		if(p->mateDp.chunk) mdp = 2 * (int)((p->maxReads + p->mateDp.chunk - 1) / p->mateDp.chunk);
 		pe = 2 + mdp;
 	}
 	return 8 + dp + pe;

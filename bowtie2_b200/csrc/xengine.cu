@@ -249,8 +249,8 @@ __global__ void __launch_bounds__(128) k_xe_report(XParams P, const XUnit *units
 }
 
 struct DpWork {                       // workspace of one DP queue (anchor rectangles / mate rectangles)
-	DpOut o{}; uint8_t *codes = nullptr; int32_t *lastH = nullptr; uint64_t *rawKeys = nullptr; uint32_t *tasks = nullptr;
-	int maxCol = 0, packed = 0, maxRaw = 0; uint64_t codeStride = 0, chunk = 0, numSlots = 0;
+	DpOut o{}; DpPlan plan{}; uint8_t *codes = nullptr; uint64_t *rawKeys = nullptr; uint32_t *tasks = nullptr;
+	int maxCol = 0; uint64_t numSlots = 0;
 };
 
 } // namespace
@@ -309,19 +309,12 @@ int setupDp(bt2g_xengine *e, DpWork &w, int maxCol, uint64_t cap, int maxCands, 
 	int64_t mn = 0;
 	for(int l = 1; l <= e->maxLen; l++) if(e->T.minsc[l] < mn) mn = e->T.minsc[l];
 	w.maxCol = maxCol + 1;
-	w.packed = sc.local ? 0 : dp_kernel_mode(sc, mn, e->maxLen, e->ctx->dpModeCap);
-	w.codeStride = dp_code_stride(w.maxCol, e->maxLen, w.packed);
 	w.numSlots = (uint64_t)e->sms * 24;
-	int rc = 0;
 	// (3 GiB of H-byte workspace per queue: each half still holds a resident round of the fill, and several engines fit one GPU)
-	if(w.packed == 3) {
-		w.chunk = dp_chunk_problems(w.codeStride, cap, 3ull << 30);
-		rc |= xalloc(e, w.codes, w.chunk * w.codeStride); rc |= xalloc(e, w.tasks, 4);
-	}
-	else rc |= xalloc(e, w.codes, w.numSlots * w.codeStride * (w.packed ? 2 : 1));
-	rc |= xalloc(e, w.lastH, w.numSlots * (uint64_t)w.maxCol);
-	w.maxRaw = maxCands * 4 < 1024 ? 1024 : maxCands * 4;
-	if(sc.local) rc |= xalloc(e, w.rawKeys, w.numSlots * (uint64_t)w.maxRaw);
+	w.plan = dp_plan(sc, mn, e->maxLen, w.maxCol, cap, w.numSlots, maxCands * 4 < 1024 ? 1024 : maxCands * 4, e->ctx->dpModeCap, 3ull << 30);
+	int rc = xalloc(e, w.codes, w.plan.codeBytes);
+	if(w.plan.taskCtr) rc |= xalloc(e, w.tasks, 4);
+	if(w.plan.rawKeys) rc |= xalloc(e, w.rawKeys, w.plan.rawKeys);
 	w.o.maxCands = maxCands; w.o.maxAlns = maxAlns; w.o.maxOps = e->maxOps;
 	rc |= xalloc(e, w.o.probs, cap); rc |= xalloc(e, w.o.summ, cap); rc |= xalloc(e, w.o.cands, cap * (uint64_t)maxCands);
 	rc |= xalloc(e, w.o.alns, cap * (uint64_t)maxAlns); rc |= xalloc(e, w.o.ops, cap * (uint64_t)maxAlns * w.o.maxOps);
@@ -334,16 +327,16 @@ int launchDp(bt2g_xengine *e, const DpWork &w, uint64_t n, cudaStream_t st, cuda
 	if(n == 0) return 0;
 	DpLaunch L;
 	L.seq = e->d.seq; L.qual = e->d.qual; L.roff = e->d.roff; L.probs = w.o.probs; L.n = n; L.nDev = nullptr;
-	L.numSlots = w.numSlots; L.codes = w.codes; L.lastH = w.lastH; L.rawKeys = w.rawKeys; L.maxRaw = w.rawKeys ? w.maxRaw : 0;
-	L.codeStride = w.codeStride; L.maxCol = w.maxCol; L.maxCands = w.o.maxCands; L.maxAlns = w.o.maxAlns; L.maxOps = w.o.maxOps;
-	L.chunk = w.chunk; L.packed = w.packed; L.taskCtr = w.tasks;
+	L.numSlots = w.numSlots; L.codes = w.codes; L.rawKeys = w.rawKeys; L.maxRaw = w.plan.maxRaw;
+	L.codeStride = w.plan.codeStride; L.maxCol = w.maxCol; L.maxCands = w.o.maxCands; L.maxAlns = w.o.maxAlns; L.maxOps = w.o.maxOps;
+	L.chunk = w.plan.chunk; L.mode = w.plan.mode; L.taskCtr = w.tasks;
 	L.st2 = st2; L.evFork = e->evFork; L.evJoin = e->evJoin;
 	uint64_t chunks = 0; L.nChunks = &chunks;
 	{ const int qi = &w == &e->M ? 1 : 0; e->tevN[qi] = 0; L.tev = e->tev[qi]; L.tevCap = XE_TEV; L.tevN = &e->tevN[qi]; }
 	L.summ = w.o.summ; L.cands = w.o.cands; L.alns = w.o.alns; L.ops = w.o.ops;
 	const DevIndex<OFF> ix = bt2g_dev_index<OFF>(e->ctx);
 	const int rc = e->sc.local ? launch_dp_local<OFF>(ix, e->sc, L, e->maxLen, st) : launch_dp_e2e<OFF>(ix, e->sc, L, e->maxLen, st);
-	e->launches += (!e->sc.local && w.packed == 3) ? 2 * chunks : 1;
+	e->launches += w.plan.mode == 3 ? 2 * chunks : 1;
 	return rc;
 }
 

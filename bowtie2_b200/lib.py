@@ -327,7 +327,8 @@ def _set_scoring_policy(self, sc, local: bool = None):
 
 
 def _set_dp_mode(self, cap: int):
-    """bt2g_set_dp_mode: cap the end-to-end DP kernel generation (0..3) of this context"""
+    """bt2g_set_dp_mode: cap the end-to-end DP kernel generation of this context: 0 (32-bit move codes), 1 (s16x2 move
+    codes), 3 (split H-byte fill + tail, the default); a cap of 2 selects what a cap of 1 does"""
     self._lib.bt2g_set_dp_mode.argtypes = [C.c_void_p, C.c_int]
     self._check(self._lib.bt2g_set_dp_mode(self._h, int(cap)), "bt2g_set_dp_mode")
 

@@ -2,12 +2,15 @@
 counts that a row block, a lane and a warp's rows divide (multiples of 16, 32, 48 and 64), chunks whose problem count leaves a
 packed slot or a warp's second pair idle, problems of very different widths side by side, a bad-shape problem among good ones,
 and a match bonus (full-width blocks).  Against the unmodified reference SwAligner with the checks of test_dp_gpu._check, or,
-with a match bonus, against the fused H-byte kernel."""
+with a match bonus, against the recorded results of the fused H-byte kernel."""
+import os
+
 import numpy as np
 import pytest
 
 from bowtie2_b200 import policy, synth
 from bowtie2_b200.lib import ReadBatch
+from conftest import GOLDEN
 from oracle_lib import Reference, have_reference
 from test_dp_gpu import _check, _problems
 from test_dp_mate_gpu import _mate_problems, mate_genome, mate_index  # noqa: F401  (fixtures)
@@ -109,26 +112,47 @@ def test_dp_bad_shape_among_good(gpu, mate_index, mate_genome, L):
     _assert_same(tuple(x[good] for x in full), gpu.dp_extend(batch, probs[good], max_cands=256, max_alns=8, max_ops=L + 80))
 
 
-@pytest.mark.parametrize("L", [15, 16, 17, 33, 47, 48, 49, 64])
-def test_dp_match_bonus_same_as_fused_kernel(gpu, mate_index, mate_genome, L, monkeypatch):
-    """With a match bonus every row block sweeps the full width; the split H-byte kernels give what the fused H-byte kernel
-    gives (the byte encoding holds these short reads' score range)."""
+MATCH_BONUS_LENGTHS = [15, 16, 17, 33, 47, 48, 49, 64]
+MATCH_BONUS_GOLDEN = os.path.join(GOLDEN, "dp_match_bonus_hbyte.npz")
+
+
+def _match_bonus_problems(mate_genome, L, monkeypatch):
+    """seed-extension and mate rectangles of reads of L bases under match bonus 1, cut to 3 (mod 4) problems"""
     _short_mates(monkeypatch, L)
-    gpu.load_index_files(mate_index)
-    gpu.set_scoring(local=False, match_bonus=1)
     sc = policy.Scoring.default(False)
     sc.match_bonus = 1
     rng = np.random.default_rng(31 + L)
     reads, quals, probs, meta = _merge(_seed_problems(mate_genome, L, sc, rng, 40), _mate_problems(mate_genome, L, sc, rng))
-    probs = probs[:len(probs) - (len(probs) - 3) % 4]                           # 3 (mod 4)
-    batch = ReadBatch.from_list(reads, quals)
-    out = {}
+    return ReadBatch.from_list(reads, quals), probs[:len(probs) - (len(probs) - 3) % 4]
+
+
+def _compact(out):
+    """everything a dp_extend result reports (the fields _assert_same compares) as four flat arrays"""
+    s, c, a, o = out
+    summ = np.stack([s[f].astype(np.int64) for f in ("found", "best", "ncand", "naln", "flags")], axis=1)
+    cands = [c[k][:int(s["ncand"][k])] for k in range(len(s))]
+    alns = [a[k][:int(s["naln"][k])] for k in range(len(s))]
+    ops = [o[k][i][:int(alns[k][i]["nops"])] for k in range(len(s)) for i in range(len(alns[k]))]
+    return {"summ": summ, "cands": np.concatenate(cands), "alns": np.concatenate(alns), "ops": np.concatenate(ops)}
+
+
+@pytest.mark.parametrize("L", MATCH_BONUS_LENGTHS)
+def test_dp_match_bonus_same_as_recorded_fused_kernel(gpu, mate_index, mate_genome, L, monkeypatch):
+    """With a match bonus every row block sweeps the full width; the split H-byte kernels give what the fused H-byte kernel gave
+    on the same problems (the byte encoding holds these short reads' score range).  tests/golden/dp_match_bonus_hbyte.npz holds
+    the fused kernel's results, recorded before it was retired.  The move-code kernels are no substitute: they report the exact
+    best score of a problem without candidates where the H-byte kernels report the floor, and end-to-end scoring with a match
+    bonus, which the reference does not define, lets their backtraces find other alignments."""
+    gpu.load_index_files(mate_index)
+    gpu.set_scoring(local=False, match_bonus=1)
+    batch, probs = _match_bonus_problems(mate_genome, L, monkeypatch)
     try:
-        for cap in (3, 2):
-            gpu.set_dp_mode(cap)
-            out[cap] = gpu.dp_extend(batch, probs, max_cands=256, max_alns=8, max_ops=L + 80)
-    finally:
         gpu.set_dp_mode(3)
+        out = gpu.dp_extend(batch, probs, max_cands=256, max_alns=8, max_ops=L + 80)
+    finally:
         gpu.set_scoring(local=False)
-    assert int(out[3][0]["found"].sum()) > 10
-    _assert_same(out[3], out[2])
+    assert int(out[0]["found"].sum()) > 10
+    got, want = _compact(out), np.load(MATCH_BONUS_GOLDEN)
+    for key, v in got.items():
+        w = want[f"{key}_{L}"]
+        assert v.dtype == w.dtype and v.shape == w.shape and v.tobytes() == w.tobytes(), key

@@ -103,11 +103,12 @@ def test_dp_e2e_matches_reference(gpu, synth_index, synth_genome, rdlen, sub, in
 
 
 @pytest.mark.skipif(not have_reference(), reason="oracle/_ref not built")
-@pytest.mark.parametrize("mode", ["0", "1", "2"])
+@pytest.mark.parametrize("mode", ["0", "1"])
 def test_dp_e2e_kernel_generations(gpu, synth_index, synth_genome, mode):
-    """The older end-to-end DP kernels (move codes 32-bit, move codes s16x2, fused H bytes) stay correct: they are the
-    fallbacks when a batch does not fit the split H-byte kernels.  The context's mode cap (bt2g_set_dp_mode) selects them: a
-    100 bp read's default minimum score fits a byte, so each cap is the mode that runs."""
+    """The move-code end-to-end DP kernels stay correct: mode 1 (s16x2) runs when a batch's score range does not fit the bytes
+    of the split H-byte kernels, mode 0 (32-bit) when it does not fit s16x2 either or under a mode cap of 0.  The context's mode
+    cap (bt2g_set_dp_mode) selects them here: a 100 bp read's default minimum score fits a byte, so each cap is the mode that
+    runs."""
     gpu.load_index_files(synth_index)
     gpu.set_scoring(local=False)
     R = Reference(synth_index)
@@ -182,12 +183,12 @@ def _kernel_mode(sc, min_minsc, max_len, cap):
     if cap == 0 or min_minsc < -8000 or sc.match_bonus * max_len > 8000:
         return 0
     rng = sc.match_bonus * max_len - (min_minsc - sc.match_bonus - 1)
-    return (3 if cap >= 3 else 2) if cap >= 2 and rng <= 127 else 1
+    return 3 if cap >= 3 and rng <= 127 else 1
 
 
 def _rows_per_lane(max_len, mode):
     """dp_rows_per_lane (dp_device.cuh); the local kernels use the move-code rows"""
-    if mode in (2, 3):
+    if mode == 3:
         return next(r for r in (4, 5, 6, 8, 10, 12, 16) if 32 * r >= max_len)
     return 4 if max_len <= 128 else (8 if max_len <= 256 else 16)
 
@@ -232,7 +233,7 @@ def _byte_bump(sc, L):
 def _caps_checked(gpu, R, genome, reads, quals, probs, meta, sc, L):
     """the problems at every mode cap (local: its one generation), each against the reference; -> found problems per cap"""
     found, wants = [], {}
-    for cap in ((3,) if sc.local else (0, 1, 2, 3)):
+    for cap in ((3,) if sc.local else (0, 1, 3)):
         gpu.set_dp_mode(cap)
         nfound, naln, _ = _check(gpu, R, genome, reads, quals, probs, meta, sc=sc, max_cands=16384 if sc.local else 2048, wants=wants)
         mode = _kernel_mode(sc, int(probs["minsc"].min()), max(len(reads[int(i)]) for i in probs["read_idx"]), cap)
@@ -266,7 +267,7 @@ def _fates(gpu, O, reads, quals, probs, meta, sc, cap):
 @pytest.mark.skipif(not have_reference(), reason="oracle/_ref not built")
 @pytest.mark.parametrize("name", sorted(scoring_grid()))
 def test_dp_matches_reference_under_scoring(gpu, synth_index, synth_genome, grid_mate_index, name):
-    """Every DP kernel generation (mode caps 0-3) at R = 4, 5, 6 and 8 on seed-extension rectangles, and on mate windows at 150 bp,
+    """Every DP kernel generation (mode caps 0, 1 and 3) at R = 4, 5, 6 and 8 on seed-extension rectangles, and on mate windows at 150 bp,
     against SwAligner under oracle_lib.scoring_grid()'s scorings; candidate fates against the C restatement's attempt log in
     modes 1 and 3 (local: its kernel)"""
     from test_dp_mate_gpu import _mate_problems
@@ -313,5 +314,5 @@ def test_dp_matches_reference_under_scoring(gpu, synth_index, synth_genome, grid
 def test_dp_zz_every_grid_generation_ran():
     """the end of the file: under the scoring grid every end-to-end generation ran with found alignments at every rows-per-lane
     instantiation that reads of 100-250 bases reach, and the local kernel at both of its"""
-    want = {(0, 4), (0, 8), (1, 4), (1, 8)} | {(m, r) for m in (2, 3) for r in (4, 5, 6, 8)} | {("local", 4), ("local", 8)}
+    want = {(0, 4), (0, 8), (1, 4), (1, 8)} | {(3, r) for r in (4, 5, 6, 8)} | {("local", 4), ("local", 8)}
     assert want <= GRID_RAN, sorted(want - GRID_RAN, key=str)

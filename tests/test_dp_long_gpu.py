@@ -5,7 +5,7 @@ lists, trims).
 The reference glue runs default penalties, so the kernel generation of a bt2g_dp_extend call is steered by the problems' minimum
 scores and the context's mode cap: under default end-to-end scoring (no match bonus) the default minimum score of a read longer than
 about 210 bases puts the whole call on the s16x2 move-code kernel (mode 1); a minimum score of -126 or more fits the score range in a
-byte, so the H-byte kernels run (mode 2 when capped at 2, the split fill + tail otherwise).  Reads of 424 bases and more have a
+byte, so the split H-byte fill + tail kernels run (mode 3) unless the cap is below 3.  Reads of 424 bases and more have a
 default minimum score below -254, where the reference leaves its u8 matrix for the i16 one; local reads longer than about 127 bases
 saturate the reference's u8 local matrix and make it rerun in i16."""
 import numpy as np
@@ -30,12 +30,12 @@ def _mode(min_minsc, cap):
     """dp_kernel_mode (dp_device.cuh) under default end-to-end scoring: no match bonus, so the range is 1 - minsc"""
     if cap == 0 or min_minsc < -8000:
         return 0
-    return (3 if cap >= 3 else 2) if cap >= 2 and 1 - min_minsc <= 127 else 1
+    return 3 if cap >= 3 and 1 - min_minsc <= 127 else 1
 
 
 def _rows(max_len, mode):
     """dp_rows_per_lane (dp_device.cuh)"""
-    if mode >= 2:
+    if mode == 3:
         return next(r for r in (4, 5, 6, 8, 10, 12, 16) if 32 * r >= max_len)
     return 4 if max_len <= 128 else (8 if max_len <= 256 else 16)
 
@@ -49,7 +49,7 @@ def _fits_four_warps(width, mode, rows):
     """whether the kernels of `mode` fit the block shapes they had before wide windows were sized (4 warps, 8 for the tail) in
     SMEM_OPTIN; max_col = width + 1, as bt2g_dp_extend counts it"""
     m = width + 1
-    if mode in (1, 2):
+    if mode == 1:
         return 4 * 2 * _smem_per_warp(m) <= SMEM_OPTIN
     if mode == 3:
         prof = (3 * 32 * rows + 15) & ~15
@@ -86,12 +86,12 @@ def _run(gpu, R, genome, reads, quals, probs, meta, cap, local=False):
     return key, got
 
 
-def _five_calls(gpu, R, genome, make):
-    """per length: default minimum score uncapped (mode 1) and capped at 0 (mode 0); a byte-range minimum score uncapped (mode 3),
-    capped at 2 (mode 2) and capped at 1 (mode 1).  make(bump) -> (reads, quals, probs, meta) with minsc = default + bump"""
+def _four_calls(gpu, R, genome, make):
+    """per length: default minimum score uncapped (mode 1) and capped at 0 (mode 0); a byte-range minimum score uncapped (mode 3)
+    and capped at 1 (mode 1).  make(bump) -> (reads, quals, probs, meta) with minsc = default + bump"""
     sc = policy.Scoring.default(False)
     keys, found = [], 0
-    for byte_range, cap in [(False, 3), (False, 0), (True, 3), (True, 2), (True, 1)]:
+    for byte_range, cap in [(False, 3), (False, 0), (True, 3), (True, 1)]:
         reads, quals, probs, meta = make(sc, byte_range)
         key, (nfound, naln, _) = _run(gpu, R, genome, reads, quals, probs, meta, cap)
         keys.append(key)
@@ -114,9 +114,8 @@ def test_long_seed_rectangles_match_reference(gpu, synth_index, synth_genome, L)
         bump = BYTE_MINSC - sc.min_score(L) if byte_range else 0
         probs, meta = _problems(synth_genome, reads, truth, sc, rng, minsc_bump=bump)
         return reads, quals, probs, meta
-    keys, _ = _five_calls(gpu, R, synth_genome, make)
-    m2 = _rows(L, 2)
-    assert keys == [(1, _rows(L, 1)), (0, _rows(L, 0)), (3, m2), (2, m2), (1, _rows(L, 1))], keys
+    keys, _ = _four_calls(gpu, R, synth_genome, make)
+    assert keys == [(1, _rows(L, 1)), (0, _rows(L, 0)), (3, _rows(L, 3)), (1, _rows(L, 1))], keys
 
 
 @pytest.mark.parametrize("L", LENGTHS)
@@ -134,8 +133,8 @@ def test_long_mate_rectangles_match_reference(gpu, mate_index, mate_genome, L):
         assert (c1 & (probs["refl"] == 0)).any() and (c1 & (probs["refr"] == len(mate_genome[1]) - 1)).any()   # windows cut at the ends
         assert ((probs["tidx"] == 0) & (probs["refl"] <= NGAP_AT) & (probs["refr"] >= NGAP_AT)).any()         # and over the N gap
         return reads, quals, probs, meta
-    keys, _ = _five_calls(gpu, R, mate_genome, make)
-    assert [k[0] for k in keys] == [1, 0, 3, 2, 1], keys
+    keys, _ = _four_calls(gpu, R, mate_genome, make)
+    assert [k[0] for k in keys] == [1, 0, 3, 1], keys
 
 
 @pytest.mark.parametrize("L", [257, 384, 512])
@@ -249,22 +248,22 @@ def _wide_problems(genome, L, W, sc, rng, byte_range):
 
 
 @pytest.mark.parametrize("L", [150, 300])
-@pytest.mark.parametrize("kind", ["mode1", "mode2", "mode3", "local"])
+@pytest.mark.parametrize("kind", ["mode1", "mode3", "local"])
 def test_wide_mate_windows_match_reference(gpu, mate_index, mate_genome, L, kind):
     """windows up to 8000 columns (the widest mate window the device engine frames) and 16000 (the coroutine engine's windows under
-    larger -X): 4000-4200 straddle the width from which 4 warps of k_dp_e2e_x2 / k_dp_e2e_h or 8 of k_dp_tail_h no longer fit one
+    larger -X): 4000-4200 straddle the width from which 4 warps of k_dp_e2e_x2 or 8 of k_dp_tail_h no longer fit one
     block's shared memory; each kernel takes fewer warps per block there, and the answers stay the reference's"""
     local = kind == "local"
     gpu.load_index_files(mate_index)
     gpu.set_scoring(local=local)
     R = Reference(mate_index)
     sc = policy.Scoring.default(local)
-    cap = {"mode1": 1, "mode2": 2, "mode3": 3, "local": 3}[kind]       # (a 150 bp read's default minsc already fits a byte)
+    cap = {"mode1": 1, "mode3": 3, "local": 3}[kind]       # (a 150 bp read's default minsc already fits a byte)
     rng = np.random.default_rng(L + len(kind))
     fits = []
     try:
         for W in WIDTHS:
-            reads, quals, probs, meta = _wide_problems(mate_genome, L, W, sc, rng, kind in ("mode2", "mode3"))
+            reads, quals, probs, meta = _wide_problems(mate_genome, L, W, sc, rng, kind == "mode3")
             assert int((probs["refr"] - probs["refl"] + 1).max()) == W
             key, (nfound, naln, _) = _run(gpu, R, mate_genome, reads, quals, probs, meta, cap, local=local)
             assert key[0] == ("local" if local else int(kind[-1])), key
@@ -283,5 +282,5 @@ def test_wide_mate_windows_match_reference(gpu, mate_index, mate_genome, L, kind
 def test_zz_every_long_kernel_instantiation_ran():
     """the end of the file: every kernel generation and rows-per-lane instantiation that reads of 251-512 bases reach ran with found
     alignments above"""
-    want = {(0, 16), (1, 8), (1, 16), (2, 10), (2, 12), (2, 16), (3, 10), (3, 12), (3, 16), ("local", 16)}
+    want = {(0, 16), (1, 8), (1, 16), (3, 10), (3, 12), (3, 16), ("local", 16)}
     assert want <= RAN, sorted(want - RAN, key=str)
